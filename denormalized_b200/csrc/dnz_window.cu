@@ -1115,7 +1115,12 @@ void dnz_window::resolve_deferred(Slot& s, const RunGeom& g, bool dirty, int64_t
     if (flags & DEFER_LIST_OVERFLOW) fail(DNZ_ERR_NOMEM, "deferred-row list overflow");
     stats.deferred_rows += (int64_t)n_in;
     if (flags & DEFER_GROUPS_FULL) {
-      uint32_t clamp = gcap;       // the device counter ran past gcap; ids >= gcap were never handed out
+      // The device counter ran past the table's capacity; ids >= gcap were never handed out, so it is pulled back to gcap.  A
+      // launch queued behind a speculative one may have overflowed a table that the replay of the earlier launch has grown
+      // since: then the counter is already below gcap and counts exactly the ids handed out; raising it to gcap would skip ids.
+      CK(cudaMemcpyAsync(h_small.p, ctl(0), 4, cudaMemcpyDeviceToHost, stream));
+      CK(cudaStreamSynchronize(stream));
+      const uint32_t clamp = std::min(*h_small.as<uint32_t>(), gcap);
       CK(cudaMemcpyAsync(ctl(0), &clamp, 4, cudaMemcpyHostToDevice, stream));
       CK(cudaStreamSynchronize(stream));
       dict_grow();

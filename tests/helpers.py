@@ -152,6 +152,109 @@ def run_oracle_batches(batches, L, S=0, filt=None):
 
 
 # ---------------------------------------------------------------------------------------------
+# kernel configurations: name -> (flags, expected_groups).  count / min / max are bit-exact by contract, so every configuration
+# must emit the same bits for the same stream.
+FLAG_FORCE_GENERIC, FLAG_NO_HINTS, FLAG_NO_QUEUE, FLAG_NO_PRIVATE, FLAG_SYNCHRONOUS = 2, 4, 8, 16, 32
+KERNEL_PATHS = {
+    "private": (0, 16),                          # 1024 groups: per-CTA private pane copies, no min/max hints
+    "hinted": (0, 0),                            # 131072 groups: hints in the dictionary slots, no private copies
+    "hinted_noqueue": (FLAG_NO_QUEUE, 0),        # colliding probes loop in place instead of the per-warp retry queue
+    "nohints": (FLAG_NO_HINTS, 0),
+    "noprivate_small": (FLAG_NO_PRIVATE, 16),    # small table without private copies: hints on a 1024-group table
+    "generic": (FLAG_FORCE_GENERIC, 0),          # no TMA-staged tiles
+    "sync": (FLAG_SYNCHRONOUS, 0),               # no speculative pipeline
+}
+
+
+def _row_order(r):
+    return (r[0], r[2] is None, r[2] or b"", r[7])
+
+
+def _row_bits(r):
+    return (r[0], r[1], r[2], r[3], bits(r[4]), bits(r[5]), r[6] is None)
+
+
+def run_paths(batches, L, S=0, filt=None, names=tuple(KERNEL_PATHS), per_batch_poll=False, want=None, **kw):
+    """Runs `batches` under each named kernel configuration, compares each with the oracle and checks that count / min / max
+    and the null flags are bit-identical between the configurations.  Returns {name: stats}."""
+    if want is None:
+        want = run_oracle_batches(batches, L, S, filt)
+    stats, ref = {}, None
+    for name in names:
+        flags, eg = KERNEL_PATHS[name]
+        got, st = run_gpu(batches, L, S, filt, per_batch_poll=per_batch_poll, flags=flags, expected_groups=eg, **kw)
+        try:
+            assert_rows_equal(got, want, check_seq=per_batch_poll)
+        except AssertionError as e:
+            raise AssertionError(f"kernel path {name!r}: {e}") from None
+        got_bits = [_row_bits(r) for r in sorted(got, key=_row_order)]
+        if ref is None:
+            ref = (name, got_bits)
+        else:
+            assert got_bits == ref[1], f"kernel paths {ref[0]!r} and {name!r} emit different bits"
+        stats[name] = st
+    return stats
+
+
+def columns_to_batch(ts, val, keys) -> Batch:
+    """Batch from a timestamp array, a value array and a list of key bytes (no nulls)."""
+    lens = np.fromiter((len(k) for k in keys), np.int64, len(keys))
+    off = np.zeros(len(keys) + 1, np.int32)
+    np.cumsum(lens, out=off[1:])
+    kb = np.frombuffer(b"".join(keys) + b"\0" * 16, np.uint8).copy()
+    return Batch(ts=np.ascontiguousarray(ts, np.int64), val=np.ascontiguousarray(val, np.float64), key_off=off, key_bytes=kb)
+
+
+def record_batch_table(rb, tag):
+    """Emitted RecordBatch -> the pyarrow Table layout of result_table(.., tag) (for assert_tables_equal)."""
+    import pyarrow as pa
+    col = {name: rb.column(i) for i, name in enumerate(rb.schema.names)}
+
+    def f64_bits(name):
+        return pa.array(np.asarray(col[name].fill_null(0.0).to_numpy(zero_copy_only=False), np.float64).view(np.int64))
+    return pa.table({"ws": col["window_start_time"].cast(pa.int64()), "key": col[rb.schema.names[0]].cast(pa.binary()),
+                     "count_" + tag: col["count"].cast(pa.int64()), "min_" + tag: f64_bits("min"), "max_" + tag: f64_bits("max"),
+                     "avg_" + tag: pa.array(np.asarray(col["average"].fill_null(0.0).to_numpy(zero_copy_only=False), np.float64)),
+                     "null_" + tag: col["min"].is_null()})
+
+
+# ---------------------------------------------------------------------------------------------
+# NumPy port of the dictionary hash of keys <= 16 B (hash_words / hash_inline in denormalized_b200/csrc/dnz_device.cuh).
+# tests/test_hash_port.py pins it against the header.
+def _rotl32(x, r):
+    return (x << np.uint32(r)) | (x >> np.uint32(32 - r))
+
+
+def hash_words(w0, w1, w2, w3, length):
+    """32-bit hash of four zero-padded little-endian key words and the key length (uint32 arrays or scalars)."""
+    w0, w1, w2, w3, length = (np.asarray(x, np.uint32) for x in (w0, w1, w2, w3, length))
+    with np.errstate(over="ignore"):
+        a, b, c = w1 * np.uint32(0xC2B2AE35), w2 * np.uint32(0x27D4EB2F), w3 * np.uint32(0x165667B1)
+        h = w0 * np.uint32(0x85EBCA6B) + _rotl32(a, 13) + _rotl32(b, 21) + _rotl32(c, 5) + length * np.uint32(0x9E3779B1)
+        h = h ^ (h >> np.uint32(16)); h = h * np.uint32(0x85EBCA6B)
+        h = h ^ (h >> np.uint32(13)); h = h * np.uint32(0xC2B2AE35)
+        h = h ^ (h >> np.uint32(16))
+    return h
+
+
+def hash_inline(k0, k1, length):
+    k0, k1 = np.asarray(k0, np.uint64), np.asarray(k1, np.uint64)
+    m = np.uint64(0xFFFFFFFF)
+    return hash_words(k0 & m, k0 >> np.uint64(32), k1 & m, k1 >> np.uint64(32), length)
+
+
+def key_words(keys):
+    """(n, 4) uint32 words of keys <= 16 B, zero padded, as the dictionary stores them."""
+    assert all(len(k) <= 16 for k in keys)
+    return np.frombuffer(b"".join(k.ljust(16, b"\0") for k in keys), "<u4").reshape(len(keys), 4)
+
+
+def hash_keys(keys):
+    w = key_words(keys)
+    return hash_words(w[:, 0], w[:, 1], w[:, 2], w[:, 3], np.fromiter((len(k) for k in keys), np.uint32, len(keys)))
+
+
+# ---------------------------------------------------------------------------------------------
 # large results: sort-free comparison (hash join on (window_start, key)) of column arrays instead of Python row tuples
 def _binary_array(key_off, key_bytes, key_isnull=None):
     import pyarrow as pa
