@@ -93,16 +93,12 @@ cudaError_t launch_pack_partials(const PackParams& p, cudaStream_t s) {
 }
 
 // ---- merge: thread per received packet ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_merge_partials(const __grid_constant__ MergeParams P) {
-  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= P.n_entries) return;
-  const PartialEntry e = P.entries[i];
-  int src = 0;
-  while (src + 1 < P.world && i >= P.src_entry_end[src]) src++;
+// Intern the packet's key (its bytes at `key`) and fold its partial state into the main pane it names.
+__device__ __forceinline__ void merge_packet(const MergeParams& P, const PartialEntry& e, const uint8_t* key) {
   uint32_t gid;
   if (e.key_len == 0xFFFFFFFFu) gid = dict_lookup_null(P.dict);
   else {
-    KeyRef k; load_key<false>(P.key_bytes + P.src_key_base[src] + e.key_off, e.key_len, k);
+    KeyRef k; load_key<false>(key, e.key_len, k);
     gid = dict_lookup(P.dict, k, false);
   }
   const int64_t pi = e.pane - P.panes.pane0;
@@ -114,6 +110,15 @@ __global__ void __launch_bounds__(256) k_merge_partials(const __grid_constant__ 
   }
   if (e.nullrows) { if (P.panes.nullrows_main[pi]) red_add_u64(P.panes.nullrows_main[pi] + gid, e.nullrows); else atomicOr(P.error, 2u); }
   if (e.fz != ~0ull) { if (P.panes.fz_main[pi]) red_min_u64(P.panes.fz_main[pi] + gid, e.fz); else atomicOr(P.error, 4u); }
+}
+
+__global__ void __launch_bounds__(256) k_merge_partials(const __grid_constant__ MergeParams P) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= P.n_entries) return;
+  const PartialEntry e = P.entries[i];
+  int src = 0;
+  while (src + 1 < P.world && i >= P.src_entry_end[src]) src++;
+  merge_packet(P, e, P.key_bytes + P.src_key_base[src] + e.key_off);
 }
 cudaError_t launch_merge_partials(const MergeParams& p, cudaStream_t s) {
   if (p.n_entries <= 0) return cudaSuccess;
@@ -215,21 +220,7 @@ __global__ void __launch_bounds__(256) k_merge_ring(const __grid_constant__ Merg
       uint4 a = __ldcg(p4), b = __ldcg(p4 + 1), c = __ldcg(p4 + 2), d = __ldcg(p4 + 3);
       memcpy(&e, &a, 16); memcpy(reinterpret_cast<char*>(&e) + 16, &b, 16); memcpy(reinterpret_cast<char*>(&e) + 32, &c, 16); memcpy(reinterpret_cast<char*>(&e) + 48, &d, 16);
     }
-    uint32_t gid;
-    if (e.key_len == 0xFFFFFFFFu) gid = dict_lookup_null(P.dict);
-    else {
-      KeyRef k; load_key<false>(keys + e.key_off, e.key_len, k);
-      gid = dict_lookup(P.dict, k, false);
-    }
-    const int64_t pi = e.pane - P.panes.pane0;
-    if (gid >= GID_DEFER_ARENA || pi < 0 || pi >= P.panes.n_panes || P.panes.main[pi] == nullptr) { atomicOr(P.error, 1u); continue; }
-    GroupState* s = P.panes.main[pi] + gid;
-    if (e.cnt) {
-      red_add_f64(&s->cnt, (double)e.cnt); red_add_f64(&s->sum, e.sum);
-      red_max_u64(&s->minkey, e.minkey); red_max_u64(&s->maxkey, e.maxkey);
-    }
-    if (e.nullrows) { if (P.panes.nullrows_main[pi]) red_add_u64(P.panes.nullrows_main[pi] + gid, e.nullrows); else atomicOr(P.error, 2u); }
-    if (e.fz != ~0ull) { if (P.panes.fz_main[pi]) red_min_u64(P.panes.fz_main[pi] + gid, e.fz); else atomicOr(P.error, 4u); }
+    merge_packet(P, e, keys + e.key_off);
   }
 }
 cudaError_t launch_merge_ring(const MergeParams& p, const XchgView& X, unsigned long long* merged_total, int sm_count, cudaStream_t s) {

@@ -791,7 +791,10 @@ __global__ void __launch_bounds__(256) k_emit(const __grid_constant__ EmitParams
   double mn = 0, mx = 0, avg = 0;
   bool agg_ok = false;
   if (P.gate) {                                       // block-uniform
-    if ((P.gate[0] | P.gate[4] | P.gate[8]) != 0ull) { if (threadIdx.x == 0 && P.blocked) *P.blocked = 1u; return; }
+    unsigned long long deferred = 0ull;
+#pragma unroll
+    for (int s = 0; s < PIPELINE_SLOTS; s++) deferred |= P.gate[s].defer_count;
+    if (deferred != 0ull) { if (threadIdx.x == 0 && P.blocked) *P.blocked = 1u; return; }
   }
   const uint32_t n_groups = min(min(*P.dict.n_groups, P.dict.gcap), P.n_groups);
   if (g < n_groups) {

@@ -1,6 +1,7 @@
 // dnz_kernels.h -- device data layout + kernel launch wrappers (internal; the public boundary is include/dnz_gpu.h)
 #pragma once
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace dnz {
@@ -72,6 +73,36 @@ struct DictView {
   unsigned long long* key_bytes_total;                                  // sum of key lengths over all groups
 };
 
+// ------------------------------------------------------------------------------------------------
+// One 256 B device control block per operator, so that a single D2H copy fetches everything the host needs after a launch.
+constexpr int PIPELINE_SLOTS = 3;     // superbatches in flight on the host side (dnz_window.h, Slot)
+struct DictCounters {                 // DictView's device counters
+  uint32_t n_groups, null_gid;
+  unsigned long long arena_used, key_bytes_total;
+};
+struct SlotCtl {                      // one pipeline slot's aggregate launch
+  unsigned long long defer_count;     // DeferList::count
+  uint32_t defer_flags;               // DeferList::flags
+  uint32_t tile_counter;              // AggParams::tile_counter
+  uint32_t emit_blocked;              // EmitParams::blocked (not cleared with the three above)
+  uint32_t pad[3];
+};
+struct ResultCursor {                 // one result set: EmitOut::cursor and EmitOut::overflow
+  unsigned long long cursor;
+  uint32_t overflow, pad;
+};
+struct CtlBlock {
+  DictCounters dict; uint8_t pad0[40];
+  SlotCtl slot[PIPELINE_SLOTS]; uint8_t pad1[32];
+  ResultCursor result[2];
+  uint32_t merge_err;                 // pane-merge / exchange-ring error flags (MergeParams::error)
+  uint32_t ts_err;                    // a timestamp string did not match the format (launch_ts_convert)
+  uint8_t pad2[24];
+};
+static_assert(sizeof(SlotCtl) == 32 && sizeof(ResultCursor) == 16, "control block entries");
+static_assert(sizeof(CtlBlock) == 256 && offsetof(CtlBlock, slot) == 64 && offsetof(CtlBlock, result) == 192 &&
+              offsetof(CtlBlock, merge_err) == 224 && offsetof(CtlBlock, ts_err) == 228, "control block layout");
+
 // Per (pane, group) partial aggregate: exactly one 32 B sector.
 struct __align__(32) GroupState {
   double cnt;                  // non-null values, kept as f64 (exact below 2^53) so that {cnt, sum} is ONE red.add.f64 pair
@@ -128,10 +159,10 @@ struct EmitParams {
   int64_t wstart, wend;
   uint32_t n_groups;             // upper bound (grid size); the kernel clamps to the device counter
   int32_t rank, world;           // multi-GPU: emit only keys with hash64 % world == rank (world <= 1: all)
-  // speculative pipeline: gate[0], gate[4], gate[8] are the deferred-row counters of the three pipeline slots (nullptr: not
-  // gated).  While any of them is non-zero some rows of an earlier launch have not been applied yet: the launch does nothing
-  // and raises *blocked so that the host issues it again after the replay.
-  const unsigned long long* gate; uint32_t* blocked;
+  // speculative pipeline: gate[0 .. PIPELINE_SLOTS) are the control block's pipeline slots (nullptr: not gated).  While any
+  // of their deferred-row counters is non-zero some rows of an earlier launch have not been applied yet: the launch does
+  // nothing and raises *blocked so that the host issues it again after the replay.
+  const SlotCtl* gate; uint32_t* blocked;
   DictView dict;
   EmitOut out;
 };

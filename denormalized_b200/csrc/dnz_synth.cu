@@ -2,6 +2,7 @@
 // (SURVEY.md §8d; value distribution of examples/examples/emit_measurements.rs:30-33,45).  Bit-identical to the
 // the host generator used by the tests (orc_synth_fill); bench/test infrastructure, not part of the hot path.
 #include "dnz_kernels.h"
+#include "dnz_window.h"
 
 namespace dnz {
 
@@ -90,3 +91,60 @@ cudaError_t launch_synth(int64_t row0, int64_t n_rows, int64_t batch_rows, uint6
 }
 
 }  // namespace dnz
+
+// ------------------------------------------------------------------------------------------------
+// C API of the generator (include/dnz_gpu.h)
+extern "C" {
+
+struct dnz_synth {
+  int dev; void* ts; void* val; void* off; void* bytes; int64_t alg_bytes;
+};
+
+int32_t dnz_synth_generate(int32_t device, int64_t row0, int64_t n_rows, int64_t batch_rows, uint64_t seed, int64_t groups,
+                           int64_t rows_per_ms, int64_t t0_ms, int32_t uuid_keys, int64_t key_mul, int64_t key_add, dnz_synth** arena,
+                           dnz_device_batch* out, int64_t n_batches) {
+  if (!arena || !out || n_rows <= 0 || batch_rows <= 0 || groups <= 0 || rows_per_ms <= 0) { g_last_error = "bad synth arguments"; return DNZ_ERR_INVALID; }
+  int64_t nb = (n_rows + batch_rows - 1) / batch_rows;
+  if (n_batches < nb) { g_last_error = "batch array too small"; return DNZ_ERR_INVALID; }
+  if (cudaSetDevice(device) != cudaSuccess) { g_last_error = "no such CUDA device"; return DNZ_ERR_CUDA; }
+  int maxlen = 36;
+  if (key_mul < 1) key_mul = 1;
+  if (!uuid_keys) { maxlen = 8; for (int64_t v = (groups - 1) * key_mul + key_add; v >= 10; v /= 10) maxlen++; }
+  int64_t off_stride = (batch_rows + 1 + 3) & ~(int64_t)3;
+  int64_t bytes_stride = (batch_rows * maxlen + 15 + 16) & ~(int64_t)15;
+  dnz_synth* a = new dnz_synth{device, nullptr, nullptr, nullptr, nullptr, 0};
+  auto bail = [&](const char* m) { g_last_error = m; dnz_synth_free(a); return DNZ_ERR_CUDA; };
+  if (cudaMalloc(&a->ts, (size_t)n_rows * 8 + 64) != cudaSuccess) return bail("cudaMalloc(ts) failed");
+  if (cudaMalloc(&a->val, (size_t)n_rows * 8 + 64) != cudaSuccess) return bail("cudaMalloc(val) failed");
+  if (cudaMalloc(&a->off, (size_t)nb * off_stride * 4 + 64) != cudaSuccess) return bail("cudaMalloc(off) failed");
+  if (cudaMalloc(&a->bytes, (size_t)nb * bytes_stride + 64) != cudaSuccess) return bail("cudaMalloc(bytes) failed");
+  if (launch_synth(row0, n_rows, batch_rows, seed, groups, rows_per_ms, t0_ms, uuid_keys, key_mul, key_add, (int64_t*)a->ts, (double*)a->val,
+                   (int32_t*)a->off, (uint8_t*)a->bytes, bytes_stride, nullptr) != cudaSuccess) return bail("synth launch failed");
+  if (cudaDeviceSynchronize() != cudaSuccess) return bail("synth kernel failed");
+  // algorithmic bytes: 20 B/row + key bytes (last offset of every batch)
+  std::vector<int32_t> last((size_t)nb);
+  for (int64_t b = 0; b < nb; b++) {
+    int64_t n = std::min(batch_rows, n_rows - b * batch_rows);
+    if (cudaMemcpy(&last[(size_t)b], (int32_t*)a->off + b * off_stride + n, 4, cudaMemcpyDeviceToHost) != cudaSuccess) return bail("memcpy failed");
+  }
+  a->alg_bytes = 20 * n_rows;
+  for (int64_t b = 0; b < nb; b++) {
+    int64_t n = std::min(batch_rows, n_rows - b * batch_rows);
+    a->alg_bytes += last[(size_t)b];
+    dnz_device_batch& d = out[b];
+    memset(&d, 0, sizeof d);
+    d.n_rows = n; d.ts = (int64_t*)a->ts + b * batch_rows; d.val = (double*)a->val + b * batch_rows;
+    d.key_off = (int32_t*)a->off + b * off_stride; d.key_bytes = (uint8_t*)a->bytes + b * bytes_stride;
+  }
+  *arena = a;
+  return DNZ_OK;
+}
+int64_t dnz_synth_bytes(const dnz_synth* a) { return a ? a->alg_bytes : 0; }
+void dnz_synth_free(dnz_synth* a) {
+  if (!a) return;
+  cudaSetDevice(a->dev);
+  cudaFree(a->ts); cudaFree(a->val); cudaFree(a->off); cudaFree(a->bytes);
+  delete a;
+}
+
+}  // extern "C"

@@ -7,69 +7,17 @@
 //                           panes shared by the L/S windows that overlap them (SURVEY.md §5.7)
 //   Dictionary          <-> GroupValues (one per frame in the reference; one per stream here, ids are stable)
 //   plan_runs           <-> the per-batch watermark rule (:255-266) + late rows re-opening emitted windows (§8a-3)
-// and the Arrow<->device buffer manager (host Arrow C-Data in, device columns, Arrow C-Data out).
-#include <cuda_runtime.h>
+// and the Arrow<->device buffer manager (host Arrow C-Data in, device columns; the way out is dnz_results.cu).  Ungrouped windows
+// finish in dnz_ungrouped.cu, the multi-GPU exchange lives in dnz_group.cu; dnz_window.h declares what they share.
+#include "dnz_window.h"
 
-#include <algorithm>
-#include <chrono>
-#include <cstdarg>
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <deque>
-#include <map>
-#include <memory>
-#include <mutex>
-#include <set>
-#include <string>
-#include <vector>
-
-#include "../../include/dnz_gpu.h"
-#include "dnz_kernels.h"
-
-using namespace dnz;
-
-namespace {
-
-struct DnzError {
-  int32_t code; std::string msg;
-};
-[[noreturn]] void fail(int32_t code, const char* fmt, ...) {
-  char buf[512]; va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-  throw DnzError{code, buf};
-}
-#define CK(expr)                                                                                          \
-  do {                                                                                                    \
-    cudaError_t e__ = (expr);                                                                             \
-    if (e__ != cudaSuccess) fail(DNZ_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
-thread_local std::string g_last_error;
-
-// DNZ_TRACE=1: host-side phase timings per superbatch on stderr (debugging aid)
-const bool g_trace = getenv("DNZ_TRACE") != nullptr;
-struct Trace {
-  std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
-  std::string line;
-  void mark(const char* what) {
-    if (!g_trace) return;
-    auto t1 = std::chrono::steady_clock::now();
-    char buf[64]; snprintf(buf, sizeof buf, " %s=%.3fms", what, std::chrono::duration<double, std::milli>(t1 - t0).count());
-    line += buf; t0 = t1;
-  }
-  void flush(const char* tag) { if (g_trace) fprintf(stderr, "[dnz] %s:%s\n", tag, line.c_str()); line.clear(); }
-};
-Trace g_tr;
-
-inline int64_t floor_div(int64_t a, int64_t b) { int64_t q = a / b; return (a % b != 0 && ((a < 0) != (b < 0))) ? q - 1 : q; }
-inline size_t round_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+namespace dnz {
 
 // ------------------------------------------------------------------------------------------------
 // device memory helpers.  All device buffers come from the CUDA stream-ordered allocator with an unbounded release
 // threshold: blocks freed by one operator stay cached in the process and are handed to the next one without a driver
 // call (plain cudaMalloc/cudaFree cost milliseconds to seconds once tens of GB are mapped, and cudaFree synchronises
 // the whole device).
-struct AllocCtx { cudaStream_t s = nullptr; bool async_ok = false; };
 AllocCtx& alloc_ctx() {
   static thread_local int cached_dev = -1; static thread_local AllocCtx* cur = nullptr;
   static std::mutex m; static std::map<int, AllocCtx> ctxs;
@@ -104,333 +52,7 @@ void dev_free(void* p) {          // callers free only after the work that used 
   if (c.async_ok) cudaFreeAsync(p, c.s); else cudaFree(p);
 }
 
-struct DevBuf {
-  void* p = nullptr; size_t bytes = 0;
-  DevBuf() = default;
-  DevBuf(const DevBuf&) = delete; DevBuf& operator=(const DevBuf&) = delete;
-  DevBuf(DevBuf&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
-  DevBuf& operator=(DevBuf&& o) noexcept { if (this != &o) { release(); p = o.p; bytes = o.bytes; o.p = nullptr; o.bytes = 0; } return *this; }
-  ~DevBuf() { release(); }
-  void release() { if (p) dev_free(p); p = nullptr; bytes = 0; }
-  void alloc(size_t n) { release(); if (n == 0) n = 256; p = dev_alloc(n); bytes = n; }
-  // grow without preserving contents
-  void reserve(size_t n) { if (n > bytes) alloc(std::max(n, bytes + bytes / 2)); }
-  // grow in stream order on `st`, keeping the first `keep` bytes: no host synchronisation (work enqueued on `st` before this call
-  // still sees the old block, which is freed behind it)
-  void regrow_on(cudaStream_t st, size_t n, size_t keep) {
-    AllocCtx& c = alloc_ctx();
-    if (!c.async_ok) {
-      DevBuf nb; nb.alloc(n);
-      if (keep && p) CK(cudaMemcpyAsync(nb.p, p, keep, cudaMemcpyDeviceToDevice, st));
-      CK(cudaStreamSynchronize(st));
-      *this = std::move(nb);
-      return;
-    }
-    void* np = nullptr;
-    CK(cudaMallocAsync(&np, n, st));
-    if (keep && p) CK(cudaMemcpyAsync(np, p, keep, cudaMemcpyDeviceToDevice, st));
-    if (p) cudaFreeAsync(p, st);
-    p = np; bytes = n;
-  }
-  template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
-
-struct PinnedBuf {
-  void* p = nullptr; size_t bytes = 0;
-  ~PinnedBuf() { if (p) cudaFreeHost(p); }
-  void reserve(size_t n) {
-    if (n <= bytes) return;
-    const size_t want = std::max(n, bytes * 2);
-    if (p) cudaFreeHost(p);
-    p = nullptr; bytes = 0;
-    CK(cudaMallocHost(&p, want)); bytes = want;
-  }
-  template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
-
-// bump allocator for the device copies of pushed host batches
-struct Arena {
-  std::vector<DevBuf> slabs; size_t cur = 0, off = 0;
-  static constexpr size_t SLAB = 256ull << 20;
-  void* alloc(size_t n) {
-    n = round_up(n + 32, 256);
-    while (true) {
-      if (cur < slabs.size() && off + n <= slabs[cur].bytes) { void* r = (char*)slabs[cur].p + off; off += n; return r; }
-      if (cur + 1 < slabs.size() && n <= slabs[cur + 1].bytes) { cur++; off = 0; continue; }
-      DevBuf b; b.alloc(std::max(n, SLAB));
-      slabs.insert(slabs.begin() + (slabs.empty() ? 0 : cur + 1), std::move(b));
-      if (slabs.size() > 1) cur++;
-      off = 0;
-    }
-  }
-  void reset() { cur = 0; off = 0; }
-};
-
-struct Pane {
-  int64_t id = 0;
-  uint64_t tag = 0;        // names this zero-initialised instance of `st` (DictSlot::hint); never reused
-  DevBuf st, nullrows, fz;
-};
-
-
-struct PendingBatch {
-  BatchDesc d{};
-  int64_t key_bytes = 0;
-  bool has_moved = false;
-  ArrowArray moved{};
-};
-
-// One superbatch (<= max_rows_per_launch rows) travelling through the pipeline.  Three of them rotate:
-//   FILLING   batches are being pushed; host batches are copied into the slot's arena as they arrive (copy stream)
-//   SEALED    the tile scan (per-batch watermarks, per-tile byte ranges) has been enqueued
-//   LAUNCHED  the aggregate launch and the emission of the windows it closes have been enqueued, a snapshot of the
-//             control block follows them in stream order
-//   FREE      the snapshot has been inspected on the host (`verify`): nothing was deferred, or it has been replayed
-// so that in steady state the host never waits between a kernel and the next one: while slot k's aggregate runs, slot k+1's
-// scan is already queued behind it and the host is one full superbatch ahead.
-constexpr int NSLOT = 3;
-struct Slot {
-  enum State { FREE, FILLING, SEALED, LAUNCHED };
-  State state = FREE;
-  int idx = 0;
-  std::vector<PendingBatch> batches; int64_t rows = 0; bool copies = false;
-  std::vector<CopyDesc> gather;       // pinned host buffers pulled by one k_gather_copy launch when the superbatch is sealed
-  Arena arena; cudaEvent_t copy_done = nullptr;
-  DevBuf d_copy_descs; PinnedBuf h_copy_descs;
-  // tile scan
-  DevBuf d_batches, d_tiles, d_minmax; PinnedBuf h_batches, h_minmax; cudaEvent_t scan_done = nullptr;
-  std::vector<BatchDesc> bds; int64_t n_tiles = 0; bool scanned = false;
-  // canonical timestamps still to be derived from raw columns of this superbatch (k_ts_convert, before the scan)
-  std::vector<TsJob> ts_jobs; int64_t ts_max_rows = 0; DevBuf d_ts_jobs; PinnedBuf h_ts_jobs;
-  // aggregate launch (its own staging: the async copies read these buffers when the stream gets there)
-  DevBuf d_ptrs, d_defer[2]; PinnedBuf h_ptrs;
-  PinnedBuf snap; cudaEvent_t done = nullptr; cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  bool timed = false; double alg_bytes = 0;
-  // what was enqueued speculatively behind the aggregate launch (replayed by verify() when rows were deferred)
-  bool speculative = false;
-  int64_t t0 = 0, t1 = 0, pmin = 0, pmax = -1;
-  std::vector<int64_t> emit_starts;
-  uint64_t add_rows_bound = 0, add_bytes_bound = 0; int emit_set = 0;
-  int64_t rows_launched = 0;
-  std::vector<std::unique_ptr<Pane>> retired;      // panes whose last window was emitted behind this launch
-  size_t ctl_off() const { return 64 + 32 * (size_t)idx; }     // defer count (u64) flags (u32) tile counter (u32) emit-blocked (u32)
-};
-
-// Device columns of emitted rows.  Two sets: emission appends to one of them; a set whose rows have all been handed out is
-// reset and becomes the next target, so a consumer that polls while input keeps streaming never makes the operator wait.
-// What may be handed out is decided by SNAPSHOTS: after every group of emit launches the cursor is copied to pinned memory
-// and an event is recorded; once the event has fired, rows below the snapshot are complete and stable (append-only).
-struct ResultSet {
-  DevBuf key_off, key_bytes, key_valid, count, mn, mx, avg, sum, agg_valid, wstart, wend;
-  uint64_t row_cap = 0, byte_cap = 0;
-  uint64_t rows = 0, bytes = 0;           // host view of the cursor: an UPPER BOUND while launches are in flight, exact after fetch_ctl
-  uint64_t exp_rows = 0, exp_bytes = 0;   // prefix already handed to the consumer
-  size_t ctl_off = 192;                   // cursor (u64) + overflow flag (u32) inside the control block
-  PinnedBuf snap; cudaEvent_t snap_ev = nullptr; bool snap_issued = false;
-};
-
-enum { COL_COUNT = 0, COL_MIN = 1, COL_MAX = 2, COL_AVG = 3, COL_SUM = 4 };
-constexpr size_t CTL_BYTES = 256, CTL_MERGE_ERR = 224, CTL_TS_ERR = 228;
-
-}  // namespace
-
-struct dnz_group;
-struct dnz_window {
-  dnz_window_config cfg{};
-  std::vector<dnz_agg> aggs; std::vector<std::string> aliases;
-  std::string key_name;
-  int key_col = -1, val_col = -1, meta_col = -1, ts_child = -1, n_input_cols = 0;
-  int ts_source = DNZ_TS_CANONICAL, ts_col = -1; TsFormat ts_fmt{};      // input-contract producer (SURVEY §8 f1)
-  int dev = 0; int sm_count = 148;
-  cudaStream_t stream = nullptr; bool own_stream = false;
-  cudaStream_t copy_stream = nullptr;
-  int64_t L = 0, S = 0, pane_ms = 0; int panes_per_window = 1;
-  int64_t max_rows = 64ll << 20;
-
-  // dictionary
-  DevBuf slots, gid_key, arena;
-  // one 256 B device control block so that a single D2H copy fetches everything the host needs after a launch:
-  //   +0    n_groups(u32) null_gid(u32) arena_used(u64) key_bytes_total(u64)
-  //   +64 + 32 s   pipeline slot s: deferred-row count(u64) flags(u32) tile counter(u32) emit-blocked(u32)
-  //   +192  result set 0: cursor(u64: rows<<32|bytes) overflow(u32);  +208 result set 1
-  //   +224  pane-merge error flags (exchange)
-  DevBuf d_ctl;
-  char* ctl(size_t off) const { return d_ctl.as<char>() + off; }
-  uint32_t dict_cap = 0, gcap = 0;
-  uint64_t arena_cap = 0;     // LOGICAL capacity handed to the kernels (<= arena.bytes): bounds what launches in flight can add
-
-  // host knowledge of the device counters: exact as of the last inspected snapshot ("known"), plus what launches enqueued since
-  // then can have added at most ("bound")
-  uint32_t n_groups_host = 0; uint64_t key_bytes_total_host = 0, arena_used_host = 0;
-  int64_t rows_since_known = 0;
-  uint64_t defer_count_host = 0; uint32_t defer_flags_host = 0;
-
-  // panes
-  std::map<int64_t, std::unique_ptr<Pane>> panes;
-  std::map<int64_t, std::unique_ptr<Pane>> late_panes;     // one-batch panes of the exact late path (alive only inside a dirty run)
-  std::vector<std::unique_ptr<Pane>> pane_pool;
-  bool need_nullrows = false, need_fz = false;
-  uint64_t next_tag = 1;   // pane instance tags (low 32 bits are stored in the hints)
-  bool has_wm = false; int64_t wm = 0;
-  int64_t emitted_upto = INT64_MIN;
-
-  // pipeline
-  Slot slot[NSLOT]; int fill = 0; int64_t next_seq = 0;
-  std::vector<int> sealed_order;      // SEALED slots, oldest first
-  std::vector<int> launched_order;    // LAUNCHED slots, oldest first
-  Slot& cur() { return slot[fill]; }
-  bool in_process = false;            // an error thrown while true kills the stream (sticky), as the reference's panics do
-
-  // scratch
-  DevBuf d_priv, d_copy_cursor;
-  PinnedBuf h_small;
-  ResultSet rs[2]; int wr = 0; bool async_polls = false;
-  ResultSet& R() { return rs[wr]; }
-  cudaStream_t d2h_stream = nullptr;
-  bool res_consumed = false;
-
-  // ungrouped windows `.window([], aggs, ..)` (SURVEY §8 f2): the device reduces rows into panes; the Partial stage's per-batch
-  // emission schedule and the whole Final stage (streaming_window.rs:882-1051) run on the host over one 40 B state per window
-  bool ungrouped = false;
-  std::set<int64_t> u_created;                  // Partial frames that exist (window starts)
-  struct UEmission { std::vector<std::vector<int64_t>> pbs; size_t first = 0, count = 0; cudaEvent_t ev = nullptr; };
-  std::deque<UEmission> u_pending;              // emissions whose partial states are on their way to the host
-  std::vector<cudaEvent_t> u_event_pool;
-  DevBuf d_uwins, d_ustates; PinnedBuf h_uwins, h_ustates; size_t u_ring = 0, u_head = 0;   // UState / UWindow slots, bump-allocated; reset when nothing is pending
-  struct UFrame { int64_t end = 0; uint64_t cnt = 0; double sum = 0; bool has = false; double mn = 0, mx = 0; };
-  std::map<int64_t, UFrame> u_final; std::set<int64_t> u_seen; bool u_has_fwm = false; int64_t u_fwm = 0;
-  struct URow { int64_t ws, we; int64_t cnt; double mn, mx, avg, sum; bool valid; };
-  std::vector<URow> u_out;
-  void ungrouped_collect(bool wait);
-  void ungrouped_final(const std::vector<URow>& pb);
-  void export_ungrouped(ArrowArray* out, ArrowSchema* schema, int32_t* has_output, bool blocking);
-
-  // multi-GPU pane exchange
-  int rank = 0, world = 1;
-  bool fused = false;                             // attached to a dnz_group: launches stay asynchronous, emission happens in the group step
-  bool group_started = false;                     // this operator has taken part in a group step (its stream has begun in the group)
-  bool has_lwm = false; int64_t lwm = 0;          // local watermark (exchange mode: emission follows the GLOBAL one)
-  int64_t exported_pane_upto = INT64_MIN;
-  DevBuf d_part_entries, d_part_keys, d_owner_cursor, d_xptrs; PinnedBuf h_xptrs;
-  std::vector<int64_t> h_owner_counts, h_owner_bytes;
-  void group_begin(struct dnz_group* g);
-  void group_pack(struct dnz_group* g);
-  void group_finish(struct dnz_group* g, int64_t* gwm_out);
-  void export_partials(int64_t watermark, dnz_partials* out);
-  void import_partials(const uint8_t* entries, const int64_t* src_counts, const uint8_t* key_bytes, const int64_t* src_key_bytes,
-                       int64_t pane_lo, int64_t pane_hi);
-
-  dnz_stats stats{};
-  std::string err; int32_t sticky = 0;
-
-  ~dnz_window();
-  void init(const dnz_window_config* c, const ArrowSchema* schema);
-  DictView dict_view() const;
-  void dict_alloc(uint32_t new_gcap);
-  void dict_grow();
-  void arena_grow(uint64_t at_least);
-  void arena_trim();
-  void fetch_ctl();
-  void parse_ctl(const char* h);
-  template <class F> void for_each_live_pane(F f);
-  Pane* get_pane(int64_t id, bool create);
-  Pane* find_pane(int64_t id);
-  std::unique_ptr<Pane> new_pane(int64_t id);
-  void ensure_side_arrays(Pane* p);
-  void retire_panes(Slot* sl);
-  void push_host(ArrowArray* batch);
-  void push_dev(const dnz_device_batch* b, int64_t n);
-  void process_pending();
-  void drain();
-  void seal_current();
-  void finish_copies(Slot& s);
-  void launch_scan(Slot& s);
-  void launch_slot(Slot& s);
-  void verify(Slot& s);
-  void release_slot(Slot& s);
-  void prealloc();
-  struct Run { size_t b0, b1; bool dirty; int64_t horizon, wm_after; };
-  void plan_runs(Slot& s, const std::vector<BatchMinMax>& mm, std::vector<Run>& runs);
-  void ungrouped_emit_run(Slot* sl, const std::vector<BatchMinMax>* mm, const Run* r, int64_t flush_wm);
-  struct RunGeom { int64_t t0 = 0, t1 = 0, pmin = INT64_MAX, pmax = INT64_MIN, rows = 0; double alg_bytes = 0; bool val_nulls = false; };
-  RunGeom run_geometry(Slot& s, const std::vector<BatchMinMax>& mm, const Run& r);
-  void prepare_panes(Slot& s, const std::vector<BatchMinMax>& mm, const Run& r, const RunGeom& g);
-  AggParams build_agg_params(Slot& s, const RunGeom& g, bool dirty, int64_t horizon, int out_list);
-  void launch_aggregate_pass(Slot& s, const RunGeom& g, AggParams& P, bool dirty);
-  void resolve_deferred(Slot& s, const RunGeom& g, bool dirty, int64_t horizon);
-  void execute_run_sync(Slot& s, const std::vector<BatchMinMax>& mm, const Run& r);
-  void emit_windows(const std::vector<int64_t>& starts, const std::map<int64_t, Pane*>& src, bool gated, Slot* sl);
-  void emit_normal(int64_t wm_new, bool gated, Slot* sl);
-  std::map<int64_t, Pane*> pane_sources();
-  void ensure_result_capacity(uint64_t add_rows, uint64_t add_bytes);
-  uint32_t groups_bound() const;
-  uint64_t key_bytes_bound() const;
-  void reset_results();
-  void reset_set(int i);
-  void snapshot_results();
-  void rotate_result_sets();
-  bool set_drained(ResultSet& r);
-  void export_arrow(ArrowArray* out, ArrowSchema* schema, int32_t* has_output, bool blocking);
-  void export_device(dnz_device_result* out, bool blocking);
-  void checkpoint(std::vector<char>& blob);
-  void restore(const char* blob, size_t bytes);
-  void fill_schema(ArrowSchema* schema);
-};
-
-namespace {
-
-// ------------------------------------------------------------------------------------------------
-// Arrow C-Data export plumbing
-// Page-locked blocks for exported results are recycled: cudaMallocHost costs milliseconds, a poll must not.
-struct PinnedPool {
-  std::mutex m; std::multimap<size_t, void*> free_blocks;
-  void* get(size_t n, size_t& cap) {
-    {
-      std::lock_guard<std::mutex> g(m);
-      auto it = free_blocks.lower_bound(n);
-      if (it != free_blocks.end() && it->first <= 4 * n + (1 << 20)) { void* p = it->second; cap = it->first; free_blocks.erase(it); return p; }
-    }
-    void* p = nullptr; cap = round_up(n + n / 4, 1 << 16);
-    CK(cudaMallocHost(&p, cap));
-    return p;
-  }
-  void put(void* p, size_t cap) {
-    std::lock_guard<std::mutex> g(m);
-    if (free_blocks.size() >= 8) { auto it = free_blocks.begin(); cudaFreeHost(it->second); free_blocks.erase(it); }
-    free_blocks.emplace(cap, p);
-  }
-};
-PinnedPool g_pinned_pool;
-
-struct ExportPrivate {
-  void* block = nullptr; size_t block_cap = 0;   // one pooled page-locked block holds every exported buffer
-  ~ExportPrivate() { if (block) g_pinned_pool.put(block, block_cap); }
-  std::vector<std::unique_ptr<ArrowArray>> children; std::vector<ArrowArray*> child_ptrs;
-  std::vector<std::vector<const void*>> buffers;
-};
-void release_array(ArrowArray* a) {
-  if (!a || !a->release) return;
-  if (a->private_data) {
-    delete static_cast<ExportPrivate*>(a->private_data);
-  }
-  a->release = nullptr;
-}
-void release_child(ArrowArray* a) { a->release = nullptr; }
-
-struct SchemaPrivate {
-  std::vector<std::unique_ptr<ArrowSchema>> children; std::vector<ArrowSchema*> child_ptrs; std::vector<std::string> names;
-};
-void release_schema(ArrowSchema* s) {
-  if (!s || !s->release) return;
-  if (s->private_data) delete static_cast<SchemaPrivate*>(s->private_data);
-  s->release = nullptr;
-}
-void release_child_schema(ArrowSchema* s) { s->release = nullptr; }
-
-const char* agg_format(int kind) { return kind == DNZ_AGG_COUNT ? "l" : "g"; }
-
-}  // namespace
-
+}  // namespace dnz
 
 // =================================================================================================
 dnz_window::~dnz_window() {
@@ -532,20 +154,19 @@ void dnz_window::init(const dnz_window_config* c, const ArrowSchema* schema) {
   else { CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking)); own_stream = true; }
   CK(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
   CK(cudaStreamCreateWithFlags(&d2h_stream, cudaStreamNonBlocking));
-  rs[0].ctl_off = 192; rs[1].ctl_off = 208;
   for (auto& r : rs) { CK(cudaEventCreateWithFlags(&r.snap_ev, cudaEventDisableTiming)); r.snap.reserve(64); }
-  for (int i = 0; i < NSLOT; i++) {
+  for (int i = 0; i < PIPELINE_SLOTS; i++) {
     Slot& s = slot[i]; s.idx = i;
     CK(cudaEventCreateWithFlags(&s.copy_done, cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&s.scan_done, cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
     CK(cudaEventCreate(&s.ev0)); CK(cudaEventCreate(&s.ev1));
-    s.snap.reserve(CTL_BYTES);
+    s.snap.reserve(sizeof(CtlBlock));
   }
   slot[0].state = Slot::FILLING; fill = 0;
   CK(agg_kernel_setup());
 
-  d_ctl.alloc(CTL_BYTES); CK(cudaMemsetAsync(d_ctl.p, 0, CTL_BYTES, stream));
+  d_ctl.alloc(sizeof(CtlBlock)); CK(cudaMemsetAsync(d_ctl.p, 0, sizeof(CtlBlock), stream));
   uint64_t eg = c->expected_groups > 0 ? (uint64_t)c->expected_groups : (1ull << 16);
   uint64_t g0 = 1024; while (g0 < eg + eg / 8) g0 <<= 1;
   if (g0 > (1ull << 29)) fail(DNZ_ERR_INVALID, "expected_groups too large");
@@ -565,10 +186,10 @@ void dnz_window::init(const dnz_window_config* c, const ArrowSchema* schema) {
 DictView dnz_window::dict_view() const {
   DictView d;
   d.slots = slots.as<DictSlot>(); d.mask = dict_cap - 1; d.gcap = gcap;
-  uint32_t* c32 = reinterpret_cast<uint32_t*>(ctl(0));
-  d.n_groups = c32; d.null_gid = c32 + 1;
-  d.arena_used = reinterpret_cast<unsigned long long*>(c32 + 2);
-  d.key_bytes_total = reinterpret_cast<unsigned long long*>(c32 + 4);
+  DictCounters* c = &ctl()->dict;
+  d.n_groups = &c->n_groups; d.null_gid = &c->null_gid;
+  d.arena_used = &c->arena_used;
+  d.key_bytes_total = &c->key_bytes_total;
   d.gid_key = gid_key.as<GidKey>();
   d.arena = arena.as<uint8_t>(); d.arena_cap = arena_cap;
   return d;
@@ -636,30 +257,30 @@ void dnz_window::arena_trim() {
   if (want < arena_cap && arena_used_host <= want) arena_cap = std::max<uint64_t>(want, 1 << 20);
 }
 
-void dnz_window::parse_ctl(const char* h) {
-  if (*reinterpret_cast<const uint32_t*>(h + CTL_TS_ERR)) fail(DNZ_ERR_DATA, "a timestamp string does not match the format (the reference unwraps the parse error and panics)");
-  if (const uint32_t xe = *reinterpret_cast<const uint32_t*>(h + CTL_MERGE_ERR)) {
+void dnz_window::parse_ctl(const CtlBlock& h) {
+  if (h.ts_err) fail(DNZ_ERR_DATA, "a timestamp string does not match the format (the reference unwraps the parse error and panics)");
+  if (const uint32_t xe = h.merge_err) {
     if (xe & 0x100u) fail(DNZ_ERR_NOMEM, "exchange ring overflow: an owner's ring is smaller than one step's packets (dnz_group_config.ring_entries / ring_key_bytes)");
     fail(DNZ_ERR_NOMEM, "pane merge failed (flags %u): the dictionary / key arena of this rank is too small for the keys it owns (in exchange mode expected_groups must cover the GLOBAL key set)", xe);
   }
-  n_groups_host = std::min(*reinterpret_cast<const uint32_t*>(h), gcap);
-  arena_used_host = *reinterpret_cast<const uint64_t*>(h + 8);
-  key_bytes_total_host = *reinterpret_cast<const uint64_t*>(h + 16);
-  for (auto& r : rs)
-    if (*reinterpret_cast<const uint32_t*>(h + r.ctl_off + 8)) fail(DNZ_ERR_NOMEM, "result buffer overflow (internal sizing error)");
+  n_groups_host = std::min(h.dict.n_groups, gcap);
+  arena_used_host = h.dict.arena_used;
+  key_bytes_total_host = h.dict.key_bytes_total;
+  for (const ResultCursor& r : h.result)
+    if (r.overflow) fail(DNZ_ERR_NOMEM, "result buffer overflow (internal sizing error)");
   stats.groups = n_groups_host;
 }
 // one small D2H + sync: every launch enqueued so far has completed, the host view becomes exact
 void dnz_window::fetch_ctl() {
-  h_small.reserve(CTL_BYTES);
-  CK(cudaMemcpyAsync(h_small.p, d_ctl.p, CTL_BYTES, cudaMemcpyDeviceToHost, stream));
+  h_small.reserve(sizeof(CtlBlock));
+  CK(cudaMemcpyAsync(h_small.p, d_ctl.p, sizeof(CtlBlock), cudaMemcpyDeviceToHost, stream));
   CK(cudaStreamSynchronize(stream));
-  const char* h = h_small.as<char>();
+  const CtlBlock& h = *h_small.as<CtlBlock>();
   parse_ctl(h);
   rows_since_known = 0;
-  for (auto& r : rs) {
-    uint64_t c = *reinterpret_cast<const uint64_t*>(h + r.ctl_off);
-    r.rows = c >> 32; r.bytes = c & 0xFFFFFFFFull;
+  for (int k = 0; k < 2; k++) {
+    const uint64_t c = h.result[k].cursor;
+    rs[k].rows = c >> 32; rs[k].bytes = c & 0xFFFFFFFFull;
   }
   for (Slot& s : slot) { s.add_rows_bound = 0; s.add_bytes_bound = 0; }
 }
@@ -715,10 +336,19 @@ void dnz_window::retire_panes(Slot* sl) {
   for (auto it = panes.begin(); it != panes.end();) {
     if (it->first * pane_ms + L <= wm) {
       if (sl) sl->retired.push_back(std::move(it->second));
-      else if (pane_pool.size() < 16) pane_pool.push_back(std::move(it->second));
+      else recycle_pane(std::move(it->second));
       it = panes.erase(it);
     } else ++it;
   }
+}
+void dnz_window::recycle_pane(std::unique_ptr<Pane> p) {
+  if (pane_pool.size() < 16) pane_pool.push_back(std::move(p));
+}
+// the one-batch panes of a dirty run, once the stream has finished with them
+void dnz_window::release_late_panes() {
+  CK(cudaStreamSynchronize(stream));
+  for (auto& kv : late_panes) recycle_pane(std::move(kv.second));
+  late_panes.clear();
 }
 // an open pane, or one that was retired behind a launch that has not been verified yet (a replay of deferred rows still needs it)
 Pane* dnz_window::find_pane(int64_t id) {
@@ -883,14 +513,13 @@ void dnz_window::finish_copies(Slot& s) {
 void dnz_window::seal_current() {
   Slot& f = cur();
   if (f.batches.empty()) return;
-  struct Guard { dnz_window* w; bool prev; ~Guard() { w->in_process = prev; } } guard{this, in_process};
-  in_process = true;
+  InProcess scope(this);
   finish_copies(f);
   launch_scan(f);
   f.state = Slot::SEALED; sealed_order.push_back(f.idx);
   while (sealed_order.size() > 1) launch_slot(slot[sealed_order.front()]);
   if ((world > 1 && !fused) || (cfg.flags & DNZ_FLAG_SYNCHRONOUS)) while (!sealed_order.empty()) launch_slot(slot[sealed_order.front()]);
-  const int next = (fill + 1) % NSLOT;
+  const int next = (fill + 1) % PIPELINE_SLOTS;
   if (slot[next].state == Slot::SEALED) launch_slot(slot[next]);
   if (slot[next].state == Slot::LAUNCHED) { while (!launched_order.empty() && slot[next].state == Slot::LAUNCHED) verify(slot[launched_order.front()]); }
   fill = next; slot[next].state = Slot::FILLING;
@@ -898,15 +527,13 @@ void dnz_window::seal_current() {
 
 // enqueue everything that has been pushed (no host wait for the results)
 void dnz_window::process_pending() {
-  struct Guard { dnz_window* w; bool prev; ~Guard() { w->in_process = prev; } } guard{this, in_process};
-  in_process = true;
+  InProcess scope(this);
   if (!cur().batches.empty()) seal_current();
   while (!sealed_order.empty()) launch_slot(slot[sealed_order.front()]);
 }
 // ... and make the host view exact: every launch verified, deferred rows replayed, input batches released
 void dnz_window::drain() {
-  struct Guard { dnz_window* w; bool prev; ~Guard() { w->in_process = prev; } } guard{this, in_process};
-  in_process = true;
+  InProcess scope(this);
   while (!sealed_order.empty()) launch_slot(slot[sealed_order.front()]);
   while (!launched_order.empty()) verify(slot[launched_order.front()]);
 }
@@ -930,7 +557,7 @@ void dnz_window::launch_scan(Slot& s) {
     s.h_ts_jobs.reserve(jb); s.d_ts_jobs.reserve(jb);
     memcpy(s.h_ts_jobs.p, s.ts_jobs.data(), jb);
     CK(cudaMemcpyAsync(s.d_ts_jobs.p, s.h_ts_jobs.p, jb, cudaMemcpyHostToDevice, stream));
-    CK(launch_ts_convert(s.d_ts_jobs.as<TsJob>(), (int)s.ts_jobs.size(), s.ts_max_rows, ts_source, ts_fmt, reinterpret_cast<uint32_t*>(ctl(CTL_TS_ERR)), stream));
+    CK(launch_ts_convert(s.d_ts_jobs.as<TsJob>(), (int)s.ts_jobs.size(), s.ts_max_rows, ts_source, ts_fmt, &ctl()->ts_err, stream));
     stats.total_launches++;
     s.ts_jobs.clear(); s.ts_max_rows = 0;
   }
@@ -954,7 +581,7 @@ void dnz_window::prealloc() {
     s.d_defer[0].reserve((size_t)std::max<int64_t>(max_rows, 1) * sizeof(DeferEntry));
   }
   d_copy_cursor.alloc(64);
-  h_small.reserve(CTL_BYTES + 64);
+  h_small.reserve(sizeof(CtlBlock) + 64);
   // low cardinality: the per-CTA private pane copies (AggParams::priv) are needed by the first launch already
   if (gcap <= 8192) d_priv.reserve(256ull << 20);
   for (int i = 0; i < std::max(panes_per_window + 2, 8) && i < 16; i++) pane_pool.push_back(new_pane(0));
@@ -1044,16 +671,16 @@ void dnz_window::prepare_panes(Slot& s, const std::vector<BatchMinMax>& mm, cons
   }
 }
 
-// pane pointer table + launch parameters of one aggregate / replay pass over the run
-AggParams dnz_window::build_agg_params(Slot& s, const RunGeom& g, bool dirty, int64_t horizon, int out_list) {
-  const int64_t np = g.pmax - g.pmin + 1;
+// The pane table of panes [p0, p1]: its 7 x n_panes pointer arrays (PaneTable's, back to back) are staged at `hp` and copied to
+// `dp` in stream order.  panes(p) names the main and the late pane of id p (either may be null).  The kernels update the side
+// arrays of every pane in the table, so those are made to exist first.
+PaneTable dnz_window::upload_pane_table(void** hp, char* dp, int64_t p0, int64_t p1, const PaneLookup& panes) {
+  const int64_t np = p1 - p0 + 1;
   const size_t pb = (size_t)np * sizeof(void*);
-  s.h_ptrs.reserve(7 * pb); s.d_ptrs.reserve(7 * pb);
-  void** hp = s.h_ptrs.as<void*>();
-  for (int64_t p = g.pmin; p <= g.pmax; p++) {
-    const size_t k = (size_t)(p - g.pmin);
-    Pane* m = (!dirty || p * pane_ms + L > horizon) ? find_pane(p) : nullptr;
-    auto lit = late_panes.find(p); Pane* l = lit == late_panes.end() ? nullptr : lit->second.get();
+  for (int64_t p = p0; p <= p1; p++) {
+    const size_t k = (size_t)(p - p0);
+    const std::pair<Pane*, Pane*> ml = panes(p);
+    Pane* m = ml.first; Pane* l = ml.second;
     if (m) ensure_side_arrays(m);
     if (l) ensure_side_arrays(l);
     hp[0 * np + k] = m ? m->st.p : nullptr; hp[1 * np + k] = l ? l->st.p : nullptr;
@@ -1061,24 +688,36 @@ AggParams dnz_window::build_agg_params(Slot& s, const RunGeom& g, bool dirty, in
     hp[4 * np + k] = m ? m->fz.p : nullptr; hp[5 * np + k] = l ? l->fz.p : nullptr;
     hp[6 * np + k] = reinterpret_cast<void*>((uintptr_t)(m ? (m->tag & 0xFFFFFFFFull) : 0));
   }
-  CK(cudaMemcpyAsync(s.d_ptrs.p, hp, 7 * pb, cudaMemcpyHostToDevice, stream));
-  CK(cudaMemsetAsync(ctl(s.ctl_off()), 0, 16, stream));        // deferred-row counter, flags, tile counter (not the emit-blocked flag)
+  CK(cudaMemcpyAsync(dp, hp, 7 * pb, cudaMemcpyHostToDevice, stream));
+  PaneTable t;
+  t.pane0 = p0; t.n_panes = (int32_t)np; t.pad = 0; t.pane_ms = pane_ms;
+  t.main = (GroupState* const*)(dp + 0 * pb); t.late = (GroupState* const*)(dp + 1 * pb);
+  t.nullrows_main = (unsigned long long* const*)(dp + 2 * pb); t.nullrows_late = (unsigned long long* const*)(dp + 3 * pb);
+  t.fz_main = (unsigned long long* const*)(dp + 4 * pb); t.fz_late = (unsigned long long* const*)(dp + 5 * pb);
+  t.tag_main = (const unsigned long long*)(dp + 6 * pb);
+  return t;
+}
+
+// pane pointer table + launch parameters of one aggregate / replay pass over the run
+AggParams dnz_window::build_agg_params(Slot& s, const RunGeom& g, bool dirty, int64_t horizon, int out_list) {
+  const size_t pb = (size_t)(g.pmax - g.pmin + 1) * sizeof(void*);
+  s.h_ptrs.reserve(7 * pb); s.d_ptrs.reserve(7 * pb);
   AggParams P;
+  P.panes = upload_pane_table(s.h_ptrs.as<void*>(), s.d_ptrs.as<char>(), g.pmin, g.pmax, [&](int64_t p) {
+    auto lit = late_panes.find(p);
+    return std::make_pair((!dirty || p * pane_ms + L > horizon) ? find_pane(p) : nullptr, lit == late_panes.end() ? nullptr : lit->second.get());
+  });
+  SlotCtl& sc = ctl()->slot[s.idx];
+  CK(cudaMemsetAsync(&sc, 0, offsetof(SlotCtl, emit_blocked), stream));        // deferred-row counter, flags, tile counter (not the emit-blocked flag)
   P.batches = s.d_batches.as<BatchDesc>(); P.tiles = s.d_tiles.as<TileDesc>(); P.tile_begin = g.t0; P.tile_end = g.t1;
   P.dict = dict_view();
   P.flags = ((cfg.flags & DNZ_FLAG_NO_HINTS) ? AGG_NO_HINTS : 0) | ((cfg.flags & DNZ_FLAG_NO_QUEUE) ? AGG_NO_QUEUE : 0);
-  char* dp = s.d_ptrs.as<char>();
-  P.panes.pane0 = g.pmin; P.panes.n_panes = (int32_t)np; P.panes.pad = 0; P.panes.pane_ms = pane_ms;
-  P.panes.main = (GroupState* const*)(dp + 0 * pb); P.panes.late = (GroupState* const*)(dp + 1 * pb);
-  P.panes.nullrows_main = (unsigned long long* const*)(dp + 2 * pb); P.panes.nullrows_late = (unsigned long long* const*)(dp + 3 * pb);
-  P.panes.fz_main = (unsigned long long* const*)(dp + 4 * pb); P.panes.fz_late = (unsigned long long* const*)(dp + 5 * pb);
-  P.panes.tag_main = (const unsigned long long*)(dp + 6 * pb);
   const size_t defer_cap = (size_t)std::max<int64_t>(g.rows, 1);
   s.d_defer[out_list].reserve(defer_cap * sizeof(DeferEntry));
   P.defer.entries = s.d_defer[out_list].as<DeferEntry>();
-  P.defer.count = reinterpret_cast<unsigned long long*>(ctl(s.ctl_off())); P.defer.cap = defer_cap;
-  P.defer.flags = reinterpret_cast<uint32_t*>(ctl(s.ctl_off() + 8));
-  P.tile_counter = reinterpret_cast<uint32_t*>(ctl(s.ctl_off() + 12));
+  P.defer.count = &sc.defer_count; P.defer.cap = defer_cap;
+  P.defer.flags = &sc.defer_flags;
+  P.tile_counter = &sc.tile_counter;
   P.priv = nullptr; P.priv_groups = 0;
   return P;
 }
@@ -1118,10 +757,10 @@ void dnz_window::resolve_deferred(Slot& s, const RunGeom& g, bool dirty, int64_t
       // The device counter ran past the table's capacity; ids >= gcap were never handed out, so it is pulled back to gcap.  A
       // launch queued behind a speculative one may have overflowed a table that the replay of the earlier launch has grown
       // since: then the counter is already below gcap and counts exactly the ids handed out; raising it to gcap would skip ids.
-      CK(cudaMemcpyAsync(h_small.p, ctl(0), 4, cudaMemcpyDeviceToHost, stream));
+      CK(cudaMemcpyAsync(h_small.p, &ctl()->dict.n_groups, 4, cudaMemcpyDeviceToHost, stream));
       CK(cudaStreamSynchronize(stream));
       const uint32_t clamp = std::min(*h_small.as<uint32_t>(), gcap);
-      CK(cudaMemcpyAsync(ctl(0), &clamp, 4, cudaMemcpyHostToDevice, stream));
+      CK(cudaMemcpyAsync(&ctl()->dict.n_groups, &clamp, 4, cudaMemcpyHostToDevice, stream));
       CK(cudaStreamSynchronize(stream));
       dict_grow();
     }
@@ -1130,7 +769,7 @@ void dnz_window::resolve_deferred(Slot& s, const RunGeom& g, bool dirty, int64_t
       // never more than the key bytes of the run): pull it back to the capacity (the tail gap stays unused) and grow by that
       const uint64_t over = arena_used_host > arena_cap ? arena_used_host - arena_cap : 0;
       const uint64_t old_cap = arena_cap;
-      CK(cudaMemcpyAsync(ctl(8), &old_cap, 8, cudaMemcpyHostToDevice, stream));
+      CK(cudaMemcpyAsync(&ctl()->dict.arena_used, &old_cap, 8, cudaMemcpyHostToDevice, stream));
       CK(cudaStreamSynchronize(stream));
       arena_grow(arena_cap + std::min<uint64_t>(over, (uint64_t)g.alg_bytes) + (1 << 20));
     }
@@ -1142,62 +781,65 @@ void dnz_window::resolve_deferred(Slot& s, const RunGeom& g, bool dirty, int64_t
     CK(launch_deferred(P, s.d_defer[in_list].as<DeferEntry>(), n_in, stream));   // replays the rows of the previous pass
     stats.total_launches++;
     fetch_ctl();
-    const char* h = h_small.as<char>() + s.ctl_off();
-    n_in = *reinterpret_cast<const uint64_t*>(h); flags = *reinterpret_cast<const uint32_t*>(h + 8);
+    const SlotCtl& h = h_small.as<CtlBlock>()->slot[s.idx];
+    n_in = h.defer_count; flags = h.defer_flags;
     in_list = out_list;
   }
   arena_trim();
 }
 
+// Enqueues the aggregate launch of one run: its panes, its pane table and its parameters.  Returns the run's geometry; nothing
+// is launched for a run without tiles (t1 <= t0) or without a valid timestamp (pmin > pmax).
+dnz_window::RunGeom dnz_window::enqueue_run(Slot& s, const std::vector<BatchMinMax>& mm, const Run& r) {
+  const RunGeom g = run_geometry(s, mm, r);
+  if (g.t1 <= g.t0 || g.pmin > g.pmax) return g;
+  prepare_panes(s, mm, r, g);
+  g_tr.mark("panes");
+  AggParams P = build_agg_params(s, g, r.dirty, r.horizon, 0);
+  launch_aggregate_pass(s, g, P, r.dirty);
+  g_tr.mark("agg_launch");
+  return g;
+}
+
+// ---- process_watermark + trigger_windows of one run.  `gate`: the slot whose launch has not been verified yet, emission is
+// gated on the device (see emit_windows); nullptr: the run's rows have all been applied, emission is not gated.
+void dnz_window::advance_and_emit(const std::vector<BatchMinMax>& mm, const Run& r, Slot* gate) {
+  if (world > 1) { if (!has_lwm || lwm <= r.wm_after) lwm = r.wm_after; has_lwm = true; }   // emission follows the GLOBAL watermark
+  else if (ungrouped) {
+    ungrouped_emit_run(gate, &mm, &r, 0);
+    if (r.dirty) release_late_panes();
+  } else {
+    if (r.dirty) {
+      // windows that were already emitted (end <= horizon) and received rows from this batch are re-opened and emitted
+      // again immediately with ONLY this batch's rows (§8a-3)
+      emit_closed(late_panes, INT64_MIN, r.horizon, nullptr);
+      release_late_panes();
+    }
+    emit_normal(r.wm_after, gate);
+  }
+  g_tr.mark("emit");
+}
+
+void dnz_window::collect_kernel_time(Slot& s) {
+  if (!s.timed) return;
+  float ms = 0; CK(cudaEventElapsedTime(&ms, s.ev0, s.ev1)); stats.agg_kernel_ms += ms; stats.agg_algorithmic_bytes += s.alg_bytes; s.timed = false;
+}
+
 // Aggregates one run and triggers, waiting for the device after the launch (late batches, several runs in one superbatch,
 // exchange mode): the path the speculative one falls back to.
 void dnz_window::execute_run_sync(Slot& s, const std::vector<BatchMinMax>& mm, const Run& r) {
-  RunGeom g = run_geometry(s, mm, r);
+  const RunGeom g = enqueue_run(s, mm, r);
   if (g.t1 <= g.t0) return;
   if (g.pmin <= g.pmax) {
-    prepare_panes(s, mm, r, g);
-    g_tr.mark("panes");
-    AggParams P = build_agg_params(s, g, r.dirty, r.horizon, 0);
-    launch_aggregate_pass(s, g, P, r.dirty);
-    g_tr.mark("agg_launch");
     fetch_ctl();
     g_tr.mark("agg_wait");
-    if (s.timed) { float ms = 0; CK(cudaEventElapsedTime(&ms, s.ev0, s.ev1)); stats.agg_kernel_ms += ms; stats.agg_algorithmic_bytes += s.alg_bytes; s.timed = false; }
-    const char* h = h_small.as<char>() + s.ctl_off();
-    defer_count_host = *reinterpret_cast<const uint64_t*>(h); defer_flags_host = *reinterpret_cast<const uint32_t*>(h + 8);
+    collect_kernel_time(s);
+    const SlotCtl& h = h_small.as<CtlBlock>()->slot[s.idx];
+    defer_count_host = h.defer_count; defer_flags_host = h.defer_flags;
     if (defer_count_host) resolve_deferred(s, g, r.dirty, r.horizon);
   }
   g_tr.mark("post_agg");
-  // ---- process_watermark + trigger_windows
-  if (ungrouped) {
-    ungrouped_emit_run(nullptr, &mm, &r, 0);
-    if (r.dirty) {
-      CK(cudaStreamSynchronize(stream));
-      for (auto& kv : late_panes) if (pane_pool.size() < 16) pane_pool.push_back(std::move(kv.second));
-      late_panes.clear();
-    }
-    g_tr.mark("emit");
-    return;
-  }
-  if (r.dirty) {
-    // windows that were already emitted (end <= horizon) and received rows from this batch are re-opened and emitted
-    // again immediately with ONLY this batch's rows (§8a-3)
-    std::set<int64_t> starts;
-    for (auto& kv : late_panes)
-      for (int j = 0; j < panes_per_window; j++) {
-        int64_t st = (kv.first - j) * pane_ms;
-        if (st >= 0 && st + L <= r.horizon) starts.insert(st);
-      }
-    std::map<int64_t, Pane*> src;
-    for (auto& kv : late_panes) src[kv.first] = kv.second.get();
-    emit_windows(std::vector<int64_t>(starts.begin(), starts.end()), src, false, nullptr);
-    CK(cudaStreamSynchronize(stream));
-    for (auto& kv : late_panes) if (pane_pool.size() < 16) pane_pool.push_back(std::move(kv.second));
-    late_panes.clear();
-  }
-  if (world > 1) { if (!has_lwm || lwm <= r.wm_after) lwm = r.wm_after; has_lwm = true; }   // emission waits for the global watermark
-  else emit_normal(r.wm_after, false, nullptr);
-  g_tr.mark("emit");
+  advance_and_emit(mm, r, nullptr);
 }
 
 // The host has the scan results of a sealed superbatch: replay the reference's per-batch watermark rule over its batches, enqueue
@@ -1227,26 +869,16 @@ void dnz_window::launch_slot(Slot& s) {
     rotate_result_sets();
     if (speculative) {
       const Run& r = runs[0];
-      RunGeom g = run_geometry(s, mm, r);
+      const RunGeom g = enqueue_run(s, mm, r);
       if (g.t1 > g.t0) {
-        if (g.pmin <= g.pmax) {
-          prepare_panes(s, mm, r, g);
-          g_tr.mark("panes");
-          AggParams P = build_agg_params(s, g, false, 0, 0);
-          launch_aggregate_pass(s, g, P, false);
-          g_tr.mark("agg_launch");
-          s.speculative = true; s.t0 = g.t0; s.t1 = g.t1; s.pmin = g.pmin; s.pmax = g.pmax; s.rows_launched = g.rows;
-        }
-        if (world > 1) { if (!has_lwm || lwm <= r.wm_after) lwm = r.wm_after; has_lwm = true; }   // fused exchange: the group step emits under the GLOBAL watermark
-        else if (ungrouped) ungrouped_emit_run(&s, &mm, &r, 0);
-        else emit_normal(r.wm_after, true, &s);
-        g_tr.mark("emit");
+        if (g.pmin <= g.pmax) { s.speculative = true; s.t0 = g.t0; s.t1 = g.t1; s.pmin = g.pmin; s.pmax = g.pmax; s.rows_launched = g.rows; }
+        advance_and_emit(mm, r, &s);
       }
     } else {
       for (const Run& r : runs) execute_run_sync(s, mm, r);
     }
   }
-  CK(cudaMemcpyAsync(s.snap.p, d_ctl.p, CTL_BYTES, cudaMemcpyDeviceToHost, stream));
+  CK(cudaMemcpyAsync(s.snap.p, d_ctl.p, sizeof(CtlBlock), cudaMemcpyDeviceToHost, stream));
   CK(cudaEventRecord(s.done, stream));
   s.state = Slot::LAUNCHED; launched_order.push_back(s.idx);
   g_tr.flush("superbatch");
@@ -1256,24 +888,24 @@ void dnz_window::launch_slot(Slot& s) {
 void dnz_window::verify(Slot& s) {
   if (s.state != Slot::LAUNCHED) return;
   CK(cudaEventSynchronize(s.done));
-  const char* h = s.snap.as<char>();
+  const CtlBlock& h = *s.snap.as<CtlBlock>();
   parse_ctl(h);
   // what later launches may have added on top of this snapshot
   rows_since_known = 0;
   bool later = false;
   for (int i : launched_order) { if (i == s.idx) { later = true; continue; } if (later) rows_since_known += slot[i].rows_launched; }
   for (int k = 0; k < 2; k++) {
-    uint64_t c = *reinterpret_cast<const uint64_t*>(h + rs[k].ctl_off);
+    const uint64_t c = h.result[k].cursor;
     uint64_t rows = c >> 32, bytes = c & 0xFFFFFFFFull;
     later = false;
     for (int i : launched_order) { if (i == s.idx) { later = true; continue; } if (later && slot[i].emit_set == k) { rows += slot[i].add_rows_bound; bytes += slot[i].add_bytes_bound; } }
     rs[k].rows = rows; rs[k].bytes = bytes;
   }
-  if (s.timed) { float ms = 0; CK(cudaEventElapsedTime(&ms, s.ev0, s.ev1)); stats.agg_kernel_ms += ms; stats.agg_algorithmic_bytes += s.alg_bytes; s.timed = false; }
+  collect_kernel_time(s);
   if (s.speculative) {
-    const char* hs = h + s.ctl_off();
-    defer_count_host = *reinterpret_cast<const uint64_t*>(hs); defer_flags_host = *reinterpret_cast<const uint32_t*>(hs + 8);
-    bool blocked = *reinterpret_cast<const uint32_t*>(hs + 16) != 0;
+    const SlotCtl& hs = h.slot[s.idx];
+    defer_count_host = hs.defer_count; defer_flags_host = hs.defer_flags;
+    bool blocked = hs.emit_blocked != 0;
     if (defer_count_host && world > 1)
       fail(DNZ_ERR_NOMEM, "fused exchange: a table overflowed while launches were in flight (%llu rows deferred); size expected_groups for the GLOBAL key set", (unsigned long long)defer_count_host);
     if (defer_count_host) {
@@ -1285,97 +917,53 @@ void dnz_window::verify(Slot& s) {
       blocked = true;
     }
     if (blocked) {
-      CK(cudaMemsetAsync(ctl(s.ctl_off() + 16), 0, 4, stream));
-      if (!s.emit_starts.empty()) emit_windows(s.emit_starts, pane_sources(), false, nullptr);
+      CK(cudaMemsetAsync(&ctl()->slot[s.idx].emit_blocked, 0, 4, stream));
+      if (!s.emit_starts.empty()) emit_windows(s.emit_starts, pane_sources(), nullptr);
     }
   }
   release_slot(s);
+}
+
+// verify every slot whose launches have completed, oldest first (never waits)
+void dnz_window::verify_completed() {
+  while (!launched_order.empty() && cudaEventQuery(slot[launched_order.front()].done) == cudaSuccess) verify(slot[launched_order.front()]);
+  cudaGetLastError();
 }
 
 void dnz_window::release_slot(Slot& s) {
   if (s.copies) cudaEventSynchronize(s.copy_done);
   for (auto& pb : s.batches) if (pb.has_moved && pb.moved.release) pb.moved.release(&pb.moved);
   s.batches.clear(); s.gather.clear(); s.ts_jobs.clear(); s.ts_max_rows = 0; s.rows = 0; s.copies = false; s.arena.reset(); s.scanned = false; s.n_tiles = 0;
-  for (auto& p : s.retired) if (pane_pool.size() < 16) pane_pool.push_back(std::move(p));
+  for (auto& p : s.retired) recycle_pane(std::move(p));
   s.retired.clear(); s.emit_starts.clear(); s.speculative = false; s.add_rows_bound = s.add_bytes_bound = 0; s.rows_launched = 0;
   auto it = std::find(launched_order.begin(), launched_order.end(), s.idx);
   if (it != launched_order.end()) launched_order.erase(it);
   s.state = Slot::FREE;
 }
 
-void dnz_window::emit_normal(int64_t wm_new, bool gated, Slot* sl) {
-  if (!has_wm || wm <= wm_new) { wm = wm_new; has_wm = true; }
+// the windows with a pane in `ps` whose end lies in (end_after, end_upto], emitted from the panes of `ps`
+void dnz_window::emit_closed(const PaneMap& ps, int64_t end_after, int64_t end_upto, Slot* gate) {
   std::set<int64_t> starts;
-  for (auto& kv : panes)
+  for (auto& kv : ps)
     for (int j = 0; j < panes_per_window; j++) {
       int64_t s = (kv.first - j) * pane_ms;
-      if (s >= 0 && s + L <= wm && s + L > emitted_upto) starts.insert(s);
+      if (s >= 0 && s + L <= end_upto && s + L > end_after) starts.insert(s);
     }
   std::map<int64_t, Pane*> src;
-  for (auto& kv : panes) src[kv.first] = kv.second.get();
-  emit_windows(std::vector<int64_t>(starts.begin(), starts.end()), src, gated, sl);
+  for (auto& kv : ps) src[kv.first] = kv.second.get();
+  emit_windows(std::vector<int64_t>(starts.begin(), starts.end()), src, gate);
+}
+
+void dnz_window::emit_normal(int64_t wm_new, Slot* gate) {
+  if (!has_wm || wm <= wm_new) { wm = wm_new; has_wm = true; }
+  emit_closed(panes, emitted_upto, wm, gate);
   emitted_upto = std::max(emitted_upto, wm);
-  retire_panes(gated ? sl : nullptr);
+  retire_panes(gate);
 }
 
-void dnz_window::ensure_result_capacity(uint64_t add_rows, uint64_t add_bytes) {
-  uint64_t need_rows = R().rows + add_rows, need_bytes = R().bytes + add_bytes;
-  if (need_bytes >= (1ull << 31) || need_rows >= (1ull << 32)) {
-    // the bound may be stale: make it exact before giving up
-    drain(); fetch_ctl();
-    need_rows = R().rows + add_rows; need_bytes = R().bytes + add_bytes;
-    if (need_bytes >= (1ull << 31)) fail(DNZ_ERR_UNSUPPORTED, "more than 2 GiB of key bytes between polls (Utf8 offsets are 32-bit); poll more often");
-  }
-  if (need_rows <= R().row_cap && need_bytes <= R().byte_cap) return;
-  auto grow = [&](DevBuf& b, size_t elem, uint64_t used, uint64_t cap) { b.regrow_on(stream, (size_t)cap * elem + 64, b.p ? (size_t)used * elem : 0); };
-  if (need_rows > R().row_cap) {
-    uint64_t cap = std::max<uint64_t>(need_rows, R().row_cap + R().row_cap / 2);
-    const uint64_t used = std::min(R().rows, R().row_cap);
-    grow(R().key_off, 4, used, cap + 1); grow(R().key_valid, 1, used, cap); grow(R().count, 8, used, cap);
-    grow(R().mn, 8, used, cap); grow(R().mx, 8, used, cap); grow(R().avg, 8, used, cap); grow(R().sum, 8, used, cap);
-    grow(R().agg_valid, 1, used, cap); grow(R().wstart, 8, used, cap); grow(R().wend, 8, used, cap);
-    R().row_cap = cap;
-  }
-  if (need_bytes > R().byte_cap) {
-    uint64_t cap = std::max<uint64_t>(need_bytes, R().byte_cap + R().byte_cap / 2);
-    grow(R().key_bytes, 1, std::min(R().bytes, R().byte_cap), cap);
-    R().byte_cap = cap;
-  }
-}
-
-void dnz_window::reset_set(int i) {
-  ResultSet& r = rs[i];
-  CK(cudaMemsetAsync(ctl(r.ctl_off), 0, 16, stream));
-  r.rows = 0; r.bytes = 0; r.exp_rows = 0; r.exp_bytes = 0; r.snap_issued = false;
-  for (Slot& s : slot) if (s.emit_set == i) { s.add_rows_bound = 0; s.add_bytes_bound = 0; }
-}
-void dnz_window::reset_results() { reset_set(wr); res_consumed = false; }
-
-// cursor of the current set -> pinned memory, in stream order behind the emit launches
-void dnz_window::snapshot_results() {
-  ResultSet& r = R();
-  CK(cudaMemcpyAsync(r.snap.p, ctl(r.ctl_off), 16, cudaMemcpyDeviceToHost, stream));
-  CK(cudaEventRecord(r.snap_ev, stream));
-  r.snap_issued = true;
-}
-// every row of the set has been handed out and nothing is in flight for it
-bool dnz_window::set_drained(ResultSet& r) {
-  if (!r.snap_issued) return r.exp_rows == r.rows;
-  if (cudaEventQuery(r.snap_ev) != cudaSuccess) { cudaGetLastError(); return false; }
-  uint64_t c = *reinterpret_cast<volatile uint64_t*>(r.snap.p);
-  return (c >> 32) == r.exp_rows;
-}
-// Called before a superbatch's emits are enqueued (only matters when the consumer uses the non-blocking poll): reuse the
-// current set in place when it is drained, else switch to the other one if that is drained, else keep appending.
-void dnz_window::rotate_result_sets() {
-  if (!async_polls) return;
-  if (set_drained(rs[wr])) { if (rs[wr].exp_rows) reset_set(wr); return; }
-  if (set_drained(rs[wr ^ 1])) { if (rs[wr ^ 1].exp_rows || rs[wr ^ 1].rows) reset_set(wr ^ 1); wr ^= 1; }
-}
-
-// One k_emit launch per window: combine its panes, apply the fused FilterExec predicate, compact.  `gated`: the launches do
-// nothing (and raise the slot's emit-blocked flag) when any pipeline slot holds deferred rows at the time they run.
-void dnz_window::emit_windows(const std::vector<int64_t>& starts, const std::map<int64_t, Pane*>& src, bool gated, Slot* sl) {
+// One k_emit launch per window: combine its panes, apply the fused FilterExec predicate, compact.  `gate` (nullptr: not gated):
+// the launches do nothing (and raise that slot's emit-blocked flag) when any pipeline slot holds deferred rows at the time they run.
+void dnz_window::emit_windows(const std::vector<int64_t>& starts, const std::map<int64_t, Pane*>& src, Slot* gate) {
   if (starts.empty()) return;
   const uint32_t ng = groups_bound();
   if (ng == 0) return;
@@ -1397,381 +985,22 @@ void dnz_window::emit_windows(const std::vector<int64_t>& starts, const std::map
     E.filter_col = cfg.has_filter ? aggs[cfg.filter_agg].kind : 0; E.filter_op = cfg.filter_op; E.filter_lit = cfg.filter_literal;
     E.wstart = s; E.wend = s + L; E.n_groups = ng; E.rank = rank; E.world = world;
     E.dict = dict_view();
-    E.gate = gated ? reinterpret_cast<const unsigned long long*>(ctl(64)) : nullptr;
-    E.blocked = gated && sl ? reinterpret_cast<uint32_t*>(ctl(sl->ctl_off() + 16)) : nullptr;
+    E.gate = gate ? ctl()->slot : nullptr;
+    E.blocked = gate ? &ctl()->slot[gate->idx].emit_blocked : nullptr;
     E.out.key_off = R().key_off.as<int32_t>(); E.out.key_bytes = R().key_bytes.as<uint8_t>(); E.out.key_valid = R().key_valid.as<uint8_t>();
     E.out.count = R().count.as<int64_t>(); E.out.mn = R().mn.as<double>(); E.out.mx = R().mx.as<double>(); E.out.avg = R().avg.as<double>();
     E.out.sum = R().sum.as<double>(); E.out.agg_valid = R().agg_valid.as<uint8_t>(); E.out.wstart = R().wstart.as<int64_t>(); E.out.wend = R().wend.as<int64_t>();
-    E.out.cursor = reinterpret_cast<unsigned long long*>(ctl(R().ctl_off)); E.out.row_cap = R().row_cap; E.out.byte_cap = R().byte_cap;
-    E.out.overflow = reinterpret_cast<uint32_t*>(ctl(R().ctl_off + 8));
+    E.out.cursor = &ctl()->result[wr].cursor; E.out.row_cap = R().row_cap; E.out.byte_cap = R().byte_cap;
+    E.out.overflow = &ctl()->result[wr].overflow;
     CK(launch_emit(E, stream));
     stats.total_launches++; stats.windows_emitted++;
   }
   R().rows += add_rows; R().bytes += add_bytes;
-  if (sl && gated) {
-    sl->emit_starts.insert(sl->emit_starts.end(), starts.begin(), starts.end());
-    sl->add_rows_bound += add_rows; sl->add_bytes_bound += add_bytes; sl->emit_set = wr;
+  if (gate) {
+    gate->emit_starts.insert(gate->emit_starts.end(), starts.begin(), starts.end());
+    gate->add_rows_bound += add_rows; gate->add_bytes_bound += add_bytes; gate->emit_set = wr;
   }
   snapshot_results();
-}
-
-// ------------------------------------------------------------------------------------------------
-void dnz_window::fill_schema(ArrowSchema* schema) {
-  auto* sp = new SchemaPrivate();
-  size_t nc = (ungrouped ? 0 : 1) + aggs.size() + 2;
-  sp->names.reserve(nc);
-  auto add = [&](const std::string& name, const char* fmt, int64_t flags) {
-    sp->names.push_back(name);
-    auto c = std::make_unique<ArrowSchema>();
-    memset(c.get(), 0, sizeof(ArrowSchema));
-    c->format = fmt; c->flags = flags; c->release = release_child_schema;
-    sp->children.push_back(std::move(c));
-  };
-  if (!ungrouped) add(key_name, "u", ARROW_FLAG_NULLABLE);
-  for (size_t i = 0; i < aggs.size(); i++) add(aliases[i], agg_format(aggs[i].kind), aggs[i].kind == DNZ_AGG_COUNT ? 0 : ARROW_FLAG_NULLABLE);
-  add("window_start_time", "tsm:", 0);     // continuous/mod.rs:42-62: Timestamp(ms, None), non-null
-  add("window_end_time", "tsm:", 0);
-  for (size_t i = 0; i < nc; i++) { sp->children[i]->name = sp->names[i].c_str(); sp->child_ptrs.push_back(sp->children[i].get()); }
-  memset(schema, 0, sizeof(*schema));
-  schema->format = "+s"; schema->name = ""; schema->n_children = (int64_t)nc; schema->children = sp->child_ptrs.data();
-  schema->release = release_schema; schema->private_data = sp;
-}
-
-
-// Hands out every emitted row that is COMPLETE on the device: per result set, the rows between what was exported before and
-// the newest snapshot whose event has fired (older set first).  `blocking` callers have synchronised the stream, so every
-// snapshot has fired; the non-blocking poll simply leaves rows of still-running emits for the next call.  The device->host
-// copies run on their own stream, never behind queued input.
-void dnz_window::export_arrow(ArrowArray* out, ArrowSchema* schema, int32_t* has_output, bool blocking) {
-  if (ungrouped) { export_ungrouped(out, schema, has_output, blocking); return; }
-  if (blocking) { CK(cudaStreamSynchronize(stream)); }
-  else {
-    while (!launched_order.empty() && cudaEventQuery(slot[launched_order.front()].done) == cudaSuccess) verify(slot[launched_order.front()]);
-    cudaGetLastError();
-  }
-  struct Range { ResultSet* r; uint64_t r0, r1, b0, b1; };
-  std::vector<Range> ranges;
-  for (int k = 0; k < 2; k++) {
-    ResultSet& r = rs[k == 0 ? (wr ^ 1) : wr];
-    if (!r.snap_issued) continue;
-    if (cudaEventQuery(r.snap_ev) != cudaSuccess) { cudaGetLastError(); continue; }
-    const volatile uint64_t* sp = reinterpret_cast<volatile uint64_t*>(r.snap.p);
-    const uint64_t c = sp[0];
-    if (static_cast<uint32_t>(sp[1])) fail(DNZ_ERR_NOMEM, "result buffer overflow (internal sizing error)");
-    const uint64_t rows = c >> 32, bytes = c & 0xFFFFFFFFull;
-    if (rows > r.exp_rows) ranges.push_back(Range{&r, r.exp_rows, rows, r.exp_bytes, bytes});
-  }
-  uint64_t n = 0, nbytes = 0;
-  for (auto& g : ranges) { n += g.r1 - g.r0; nbytes += g.b1 - g.b0; }
-  if (nbytes >= (1ull << 31)) fail(DNZ_ERR_UNSUPPORTED, "more than 2 GiB of key bytes in one poll (Utf8 offsets are 32-bit); poll more often");
-  auto* ep = new ExportPrivate();
-  std::unique_ptr<ExportPrivate> guard(ep);
-  const size_t total = round_up((n + 1) * 4, 64) + round_up(nbytes, 64) + 2 * round_up(n, 64) + 7 * round_up(n * 8, 64) +
-                       2 * round_up((n + 7) / 8 + 8, 64) + 1024;
-  ep->block = g_pinned_pool.get(total, ep->block_cap);
-  size_t used = 0;
-  auto pinned = [&](size_t bytes) -> void* { void* p = (char*)ep->block + used; used += round_up(std::max<size_t>(bytes, 8), 64); return p; };
-  // one column of every range, back to back
-  auto fetch = [&](DevBuf ResultSet::*col, size_t elem, bool by_bytes, size_t extra) -> void* {
-    char* h = (char*)pinned((by_bytes ? nbytes : n) * elem + extra);
-    size_t at = 0;
-    for (auto& g : ranges) {
-      const uint64_t lo = by_bytes ? g.b0 : g.r0, hi = by_bytes ? g.b1 : g.r1;
-      const size_t bytes = (size_t)(hi - lo) * elem;
-      if (bytes) { CK(cudaMemcpyAsync(h + at, (g.r->*col).template as<char>() + lo * elem, bytes, cudaMemcpyDeviceToHost, d2h_stream)); stats.d2h_bytes += (int64_t)bytes; }
-      at += bytes;
-    }
-    return h;
-  };
-  int32_t* koff = (int32_t*)fetch(&ResultSet::key_off, 4, false, 4);
-  uint8_t* kbytes = (uint8_t*)fetch(&ResultSet::key_bytes, 1, true, 0);
-  uint8_t* kvalid = (uint8_t*)fetch(&ResultSet::key_valid, 1, false, 0);
-  int64_t* count = (int64_t*)fetch(&ResultSet::count, 8, false, 0);
-  double* mn = (double*)fetch(&ResultSet::mn, 8, false, 0); double* mx = (double*)fetch(&ResultSet::mx, 8, false, 0);
-  double* avg = (double*)fetch(&ResultSet::avg, 8, false, 0); double* sum = (double*)fetch(&ResultSet::sum, 8, false, 0);
-  uint8_t* avalid = (uint8_t*)fetch(&ResultSet::agg_valid, 1, false, 0);
-  int64_t* ws = (int64_t*)fetch(&ResultSet::wstart, 8, false, 0); int64_t* we = (int64_t*)fetch(&ResultSet::wend, 8, false, 0);
-  CK(cudaStreamSynchronize(d2h_stream));
-  {   // key offsets are relative to each set's byte buffer: rebase them onto the concatenated export
-    uint64_t row_at = 0, byte_at = 0;
-    for (auto& g : ranges) {
-      const int64_t delta = (int64_t)byte_at - (int64_t)g.b0;
-      if (delta != 0) for (uint64_t i = row_at; i < row_at + (g.r1 - g.r0); i++) koff[i] = (int32_t)(koff[i] + delta);
-      row_at += g.r1 - g.r0; byte_at += g.b1 - g.b0;
-    }
-  }
-  koff[n] = (int32_t)nbytes;
-  // byte-per-row validity -> Arrow bitmaps
-  auto pack = [&](const uint8_t* v, int64_t& nulls) -> uint8_t* {
-    nulls = 0;
-    for (uint64_t i = 0; i < n; i++) nulls += !v[i];
-    if (!nulls) return nullptr;
-    uint8_t* bm = (uint8_t*)pinned((n + 7) / 8 + 8);
-    memset(bm, 0, (n + 7) / 8 + 8);
-    for (uint64_t i = 0; i < n; i++) if (v[i]) bm[i >> 3] |= (uint8_t)(1u << (i & 7));
-    return bm;
-  };
-  int64_t key_nulls = 0, agg_nulls = 0;
-  uint8_t* kbm = pack(kvalid, key_nulls);
-  uint8_t* abm = pack(avalid, agg_nulls);
-  size_t nc = 1 + aggs.size() + 2;
-  auto add_child = [&](std::vector<const void*> bufs, int64_t nulls) {
-    ep->buffers.push_back(std::move(bufs));
-    auto c = std::make_unique<ArrowArray>();
-    memset(c.get(), 0, sizeof(ArrowArray));
-    c->length = (int64_t)n; c->null_count = nulls; c->n_buffers = (int64_t)ep->buffers.back().size();
-    c->buffers = ep->buffers.back().data(); c->release = release_child;
-    ep->children.push_back(std::move(c));
-  };
-  ep->buffers.reserve(nc + 1);
-  add_child({kbm, koff, kbytes}, key_nulls);
-  for (auto& a : aggs) {
-    switch (a.kind) {
-      case DNZ_AGG_COUNT: add_child({nullptr, count}, 0); break;
-      case DNZ_AGG_MIN: add_child({abm, mn}, agg_nulls); break;
-      case DNZ_AGG_MAX: add_child({abm, mx}, agg_nulls); break;
-      case DNZ_AGG_AVG: add_child({abm, avg}, agg_nulls); break;
-      default: add_child({abm, sum}, agg_nulls); break;
-    }
-  }
-  add_child({nullptr, ws}, 0);
-  add_child({nullptr, we}, 0);
-  for (auto& c : ep->children) ep->child_ptrs.push_back(c.get());
-  ep->buffers.push_back({nullptr});
-  memset(out, 0, sizeof(*out));
-  out->length = (int64_t)n; out->null_count = 0; out->n_buffers = 1; out->buffers = ep->buffers.back().data();
-  out->n_children = (int64_t)nc; out->children = ep->child_ptrs.data(); out->release = release_array;
-  out->private_data = guard.release();
-  if (schema) fill_schema(schema);
-  if (has_output) *has_output = n > 0;
-  stats.rows_out += (int64_t)n;
-  for (auto& g : ranges) { g.r->exp_rows = g.r1; g.r->exp_bytes = g.b1; }
-  if (blocking) {         // stream idle: drained sets can be recycled right away
-    for (int i = 0; i < 2; i++) if (rs[i].exp_rows && set_drained(rs[i])) reset_set(i);
-  }
-}
-
-// Device-resident hand-over: the oldest range of emitted rows that has not been handed out yet, one result set per call (call
-// again until n_rows == 0 when both sets may hold rows).  blocking: everything has been aggregated and the stream is idle, so
-// every emitted row is eligible.  Non-blocking: only rows whose emission is COMPLETE on the device; nothing queued is forced.
-// key_off entries are offsets into `key_bytes` (the set's byte buffer); key_bytes_len is the offset at which the last returned
-// key ends.
-void dnz_window::export_device(dnz_device_result* out, bool blocking) {
-  if (ungrouped) fail(DNZ_ERR_UNSUPPORTED, "ungrouped windows finish on the host (Final stage): use dnz_window_poll / dnz_window_poll_ready");
-  memset(out, 0, sizeof *out);
-  ResultSet* r = nullptr; uint64_t r0 = 0, r1 = 0, b1 = 0;
-  if (blocking) fetch_ctl();
-  else {
-    // release the input of launches that have completed (never waits)
-    while (!launched_order.empty() && cudaEventQuery(slot[launched_order.front()].done) == cudaSuccess) verify(slot[launched_order.front()]);
-    cudaGetLastError();
-  }
-  for (int k = 0; k < 2 && !r; k++) {
-    ResultSet& c = rs[k == 0 ? (wr ^ 1) : wr];
-    uint64_t rows = c.rows, bytes = c.bytes;
-    if (!blocking) {
-      if (!c.snap_issued) continue;
-      if (cudaEventQuery(c.snap_ev) != cudaSuccess) { cudaGetLastError(); continue; }
-      const volatile uint64_t* sp = reinterpret_cast<volatile uint64_t*>(c.snap.p);
-      const uint64_t cur = sp[0];
-      if (static_cast<uint32_t>(sp[1])) fail(DNZ_ERR_NOMEM, "result buffer overflow (internal sizing error)");
-      rows = cur >> 32; bytes = cur & 0xFFFFFFFFull;
-    }
-    if (rows > c.exp_rows) { r = &c; r0 = c.exp_rows; r1 = rows; b1 = bytes; }
-  }
-  if (!r) return;
-  r->exp_rows = r1; r->exp_bytes = b1;
-  if (blocking) {          // stream idle: a set that has been handed out completely restarts at row 0 with the next emission
-    for (int i = 0; i < 2; i++) if (rs[i].exp_rows && rs[i].exp_rows == rs[i].rows) reset_set(i);
-  }
-  out->n_rows = (int64_t)(r1 - r0); out->key_bytes_len = (int64_t)b1;
-  out->key_off = r->key_off.as<int32_t>() + r0; out->key_bytes = r->key_bytes.as<uint8_t>(); out->key_valid = r->key_valid.as<uint8_t>() + r0;
-  out->count = r->count.as<int64_t>() + r0; out->min = r->mn.as<double>() + r0; out->max = r->mx.as<double>() + r0;
-  out->avg = r->avg.as<double>() + r0; out->sum = r->sum.as<double>() + r0; out->agg_valid = r->agg_valid.as<uint8_t>() + r0;
-  out->window_start_ms = r->wstart.as<int64_t>() + r0; out->window_end_ms = r->wend.as<int64_t>() + r0;
-  stats.rows_out += (int64_t)(r1 - r0);
-}
-
-
-// ------------------------------------------------------------------------------------------------
-
-// ------------------------------------------------------------------------------------------------
-// ungrouped windows (include/dnz_gpu.h, DNZ_NO_KEY)
-namespace {
-// get_windows_for_watermark (streaming_window.rs:1053-1086), whole-second snap (:1088-1094): the frames a batch creates
-void reference_windows(int64_t mn, int64_t mx, int64_t L, int64_t S, std::vector<int64_t>& out) {
-  auto snap = [&](int64_t ts) { const int64_t wl = L / 1000, t = ts / 1000; return (t / wl) * wl * 1000; };
-  if (S > 0) { for (int64_t cur = snap(mn - L); cur <= mx; cur += S) { const int64_t end = cur + L; if (mn > end || mx < cur) continue; out.push_back(cur); } }
-  else for (int64_t cur = snap(mn); cur <= mx; cur += L) out.push_back(cur);
-}
-inline unsigned long long unord_bits_h(unsigned long long o) { return (o & 0x8000000000000000ull) ? (o & ~0x8000000000000000ull) : ~o; }
-inline int total_cmp_d(double a, double b) {
-  long long x, y; memcpy(&x, &a, 8); memcpy(&y, &b, 8);
-  x ^= (long long)(((unsigned long long)(x >> 63)) >> 1); y ^= (long long)(((unsigned long long)(y >> 63)) >> 1);
-  return x < y ? -1 : x > y ? 1 : 0;
-}
-}  // namespace
-
-// The Partial stage's emission schedule for one run (or a flush): per batch, the frames it creates and the frames its watermark
-// closes -- one "partial batch" (PB) per batch, exactly what WindowAggStream::trigger_windows hands to the Final stage -- and the
-// collection of the closed windows' states from the device (one kernel + one small D2H per run).
-void dnz_window::ungrouped_emit_run(Slot* sl, const std::vector<BatchMinMax>* mm, const Run* r, int64_t flush_wm) {
-  UEmission em;
-  std::vector<std::pair<int64_t, bool>> wins;          // (window start, from the late panes)
-  auto close_upto = [&](int64_t w, int64_t horizon, bool dirty) {
-    std::vector<int64_t> pb;
-    for (auto it = u_created.begin(); it != u_created.end();) {
-      if (*it + L <= w) { pb.push_back(*it); wins.emplace_back(*it, dirty && *it + L <= horizon); it = u_created.erase(it); } else ++it;
-    }
-    if (!pb.empty()) em.pbs.push_back(std::move(pb));
-  };
-  if (r) {
-    std::vector<int64_t> tmp;
-    for (size_t i = r->b0; i < r->b1; i++) {
-      const BatchMinMax& b = (*mm)[i];
-      if (b.n_valid == 0) continue;
-      tmp.clear(); reference_windows(b.ts_min, b.ts_max, L, S, tmp);
-      for (int64_t st : tmp) u_created.insert(st);
-      if (!has_wm || wm <= b.ts_min) { wm = b.ts_min; has_wm = true; }       // process_watermark
-      close_upto(wm, r->horizon, r->dirty);
-    }
-  } else {                                             // dnz_window_flush (tests): one trigger at the given watermark
-    if (!has_wm || wm <= flush_wm) { wm = flush_wm; has_wm = true; }
-    close_upto(wm, 0, false);
-  }
-  if (!wins.empty()) {
-    const size_t n = wins.size();
-    if (n > u_ring) fail(DNZ_ERR_UNSUPPORTED, "%zu windows closed by one run (limit %zu)", n, u_ring);
-    if (u_head + n > u_ring) { ungrouped_collect(true); u_head = 0; }              // staging full: take in what is on its way first
-    const size_t at = u_head;
-    UWindow* hw = h_uwins.as<UWindow>() + at;
-    for (size_t i = 0; i < n; i++) {
-      UWindow& W = hw[i]; memset(&W, 0, sizeof W);
-      const int64_t p0 = wins[i].first / pane_ms;
-      W.n = panes_per_window;
-      for (int j = 0; j < panes_per_window; j++) {
-        Pane* pn = nullptr;
-        if (wins[i].second) { auto it = late_panes.find(p0 + j); if (it != late_panes.end()) pn = it->second.get(); }
-        else pn = find_pane(p0 + j);
-        W.st[j] = pn ? pn->st.as<GroupState>() : nullptr; W.nr[j] = pn ? pn->nullrows.as<unsigned long long>() : nullptr;
-      }
-    }
-    CK(cudaMemcpyAsync(d_uwins.as<UWindow>() + at, hw, n * sizeof(UWindow), cudaMemcpyHostToDevice, stream));
-    CK(launch_ungrouped_collect(d_uwins.as<UWindow>() + at, (int)n, d_ustates.as<UState>() + at, stream)); stats.total_launches++;
-    CK(cudaMemcpyAsync(h_ustates.as<UState>() + at, d_ustates.as<UState>() + at, n * sizeof(UState), cudaMemcpyDeviceToHost, stream));
-    if (u_event_pool.empty()) { cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); u_event_pool.push_back(e); }
-    em.ev = u_event_pool.back(); u_event_pool.pop_back();
-    CK(cudaEventRecord(em.ev, stream));
-    em.first = at; em.count = n; u_head += n;
-    stats.windows_emitted += (int64_t)n;
-    u_pending.push_back(std::move(em));
-  }
-  emitted_upto = std::max(emitted_upto, wm);
-  retire_panes(sl);
-}
-
-// FullWindowAggStream::poll_next_inner (streaming_window.rs:934-1032) for one partial batch
-void dnz_window::ungrouped_final(const std::vector<URow>& pb) {
-  if (pb.empty()) return;
-  int64_t start = pb[0].ws, end = pb[0].we;
-  for (const URow& x : pb) { start = std::max(start, x.ws); end = std::max(end, x.we); }      // "these batches should only have 1 row"
-  const bool cached = u_final.count(start) != 0;
-  if (u_seen.count(start) && !cached) return;                                                // late data for a finalized window: dropped
-  UFrame& f = u_final[start];
-  if (!cached) f.end = end;
-  u_seen.insert(start);
-  for (const URow& x : pb) {                               // merge_batch of every row of the batch into THAT frame
-    f.cnt += (uint64_t)x.cnt;
-    if (x.valid) {
-      f.sum += x.sum;
-      if (!f.has) { f.mn = x.mn; f.mx = x.mx; f.has = true; }
-      else { if (total_cmp_d(x.mn, f.mn) < 0) f.mn = x.mn; if (total_cmp_d(x.mx, f.mx) > 0) f.mx = x.mx; }
-    }
-  }
-  if (!u_has_fwm || start > u_fwm) { u_fwm = start; u_has_fwm = true; }
-  for (auto it = u_final.begin(); it != u_final.end();) {                                    // finalize_windows: watermark > window end
-    if (u_fwm > it->second.end) {
-      const UFrame& g = it->second;
-      u_out.push_back(URow{it->first, g.end, (int64_t)g.cnt, g.has ? g.mn : 0.0, g.has ? g.mx : 0.0, g.has ? g.sum / (double)g.cnt : 0.0, g.sum, g.has});
-      it = u_final.erase(it);
-    } else ++it;
-  }
-}
-
-// feed the partial batches whose states have arrived to the Final stage (in emission order)
-void dnz_window::ungrouped_collect(bool wait) {
-  while (!u_pending.empty()) {
-    UEmission& em = u_pending.front();
-    if (wait) CK(cudaEventSynchronize(em.ev));
-    else if (cudaEventQuery(em.ev) != cudaSuccess) { cudaGetLastError(); break; }
-    const UState* st = h_ustates.as<UState>() + em.first;
-    size_t k = 0;
-    for (const auto& pb : em.pbs) {
-      std::vector<URow> rows;
-      for (int64_t ws : pb) {
-        const UState& u = st[k++];
-        URow x; x.ws = ws; x.we = ws + L; x.cnt = (int64_t)u.cnt; x.valid = u.cnt != 0; x.sum = u.sum; x.avg = 0;
-        unsigned long long bmn = unord_bits_h(~u.mink), bmx = unord_bits_h(u.maxk);
-        memcpy(&x.mn, &bmn, 8); memcpy(&x.mx, &bmx, 8);
-        rows.push_back(x);
-      }
-      ungrouped_final(rows);
-    }
-    u_event_pool.push_back(em.ev);
-    u_pending.pop_front();
-    if (u_pending.empty()) u_head = 0;
-  }
-}
-
-void dnz_window::export_ungrouped(ArrowArray* out, ArrowSchema* schema, int32_t* has_output, bool blocking) {
-  if (blocking) CK(cudaStreamSynchronize(stream));
-  else { while (!launched_order.empty() && cudaEventQuery(slot[launched_order.front()].done) == cudaSuccess) verify(slot[launched_order.front()]); cudaGetLastError(); }
-  ungrouped_collect(blocking);
-  const size_t n = u_out.size();
-  auto* ep = new ExportPrivate();
-  std::unique_ptr<ExportPrivate> guard(ep);
-  const size_t total = 8 * round_up(n * 8 + 8, 64) + round_up((n + 7) / 8 + 8, 64) + 1024;
-  ep->block = g_pinned_pool.get(total, ep->block_cap);
-  size_t used = 0;
-  auto take = [&](size_t bytes) -> void* { void* p = (char*)ep->block + used; used += round_up(std::max<size_t>(bytes, 8), 64); return p; };
-  int64_t* cnt = (int64_t*)take(n * 8); double* mn = (double*)take(n * 8); double* mx = (double*)take(n * 8); double* avg = (double*)take(n * 8);
-  double* sum = (double*)take(n * 8); int64_t* ws = (int64_t*)take(n * 8); int64_t* we = (int64_t*)take(n * 8);
-  uint8_t* bm = (uint8_t*)take((n + 7) / 8 + 8); memset(bm, 0, (n + 7) / 8 + 8);
-  int64_t nulls = 0;
-  for (size_t i = 0; i < n; i++) {
-    const URow& x = u_out[i];
-    cnt[i] = x.cnt; mn[i] = x.mn; mx[i] = x.mx; avg[i] = x.avg; sum[i] = x.valid ? x.sum : 0.0; ws[i] = x.ws; we[i] = x.we;
-    if (x.valid) bm[i >> 3] |= (uint8_t)(1u << (i & 7)); else nulls++;
-  }
-  uint8_t* abm = nulls ? bm : nullptr;
-  auto add_child = [&](std::vector<const void*> bufs, int64_t nl) {
-    ep->buffers.push_back(std::move(bufs));
-    auto c = std::make_unique<ArrowArray>(); memset(c.get(), 0, sizeof(ArrowArray));
-    c->length = (int64_t)n; c->null_count = nl; c->n_buffers = (int64_t)ep->buffers.back().size();
-    c->buffers = ep->buffers.back().data(); c->release = release_child;
-    ep->children.push_back(std::move(c));
-  };
-  ep->buffers.reserve(aggs.size() + 4);
-  for (auto& a : aggs) {
-    switch (a.kind) {
-      case DNZ_AGG_COUNT: add_child({nullptr, cnt}, 0); break;
-      case DNZ_AGG_MIN: add_child({abm, mn}, nulls); break;
-      case DNZ_AGG_MAX: add_child({abm, mx}, nulls); break;
-      case DNZ_AGG_AVG: add_child({abm, avg}, nulls); break;
-      default: add_child({abm, sum}, nulls); break;
-    }
-  }
-  add_child({nullptr, ws}, 0); add_child({nullptr, we}, 0);
-  for (auto& c : ep->children) ep->child_ptrs.push_back(c.get());
-  ep->buffers.push_back({nullptr});
-  memset(out, 0, sizeof(*out));
-  out->length = (int64_t)n; out->n_buffers = 1; out->buffers = ep->buffers.back().data();
-  out->n_children = (int64_t)ep->children.size(); out->children = ep->child_ptrs.data(); out->release = release_array;
-  out->private_data = guard.release();
-  if (schema) fill_schema(schema);
-  if (has_output) *has_output = n > 0;
-  stats.rows_out += (int64_t)n;
-  u_out.clear();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1793,13 +1022,12 @@ void dnz_window::checkpoint(std::vector<char>& blob) {
   process_pending(); drain();
   fetch_ctl();
   for (auto& r : rs) if (r.rows > r.exp_rows) fail(DNZ_ERR_INVALID, "checkpoint with emitted rows that have not been polled");
-  const char* h = h_small.as<char>();
   CkptHeader H; memset(&H, 0, sizeof H);
   memcpy(H.magic, "DNZCKPT1", 8);
   H.window_ms = L; H.slide_ms = S; H.n_aggs = (int32_t)aggs.size();
   H.flags = (has_wm ? 1 : 0) | (need_nullrows ? 2 : 0) | (need_fz ? 4 : 0) | (has_lwm ? 8 : 0);
   H.wm = wm; H.emitted_upto = emitted_upto; H.next_seq = next_seq; H.lwm = lwm; H.exported_pane_upto = exported_pane_upto;
-  H.n_groups = n_groups_host; H.null_gid_plus1 = *reinterpret_cast<const uint32_t*>(h + 4);
+  H.n_groups = n_groups_host; H.null_gid_plus1 = h_small.as<CtlBlock>()->dict.null_gid;
   H.arena_used = std::min<uint64_t>(arena_used_host, arena_cap); H.key_bytes_total = key_bytes_total_host;
   H.n_panes = (int64_t)panes.size();
   const size_t ng = H.n_groups, ab = round_up(H.arena_used, 8);
@@ -1834,8 +1062,8 @@ void dnz_window::restore(const char* blob, size_t bytes) {
   if (ab + (1 << 20) > arena_cap) arena_grow(ab + (1 << 20));
   need(ng * sizeof(GidKey)); if (ng) CK(cudaMemcpy(gid_key.p, p, ng * sizeof(GidKey), cudaMemcpyHostToDevice)); p += ng * sizeof(GidKey);
   need(ab); if (ab) CK(cudaMemcpy(arena.p, p, ab, cudaMemcpyHostToDevice)); p += ab;
-  struct { uint32_t n_groups, null_gid; uint64_t arena_used, key_bytes_total; } c0{H.n_groups, 0u, H.arena_used, H.key_bytes_total};
-  CK(cudaMemcpy(ctl(0), &c0, sizeof c0, cudaMemcpyHostToDevice));
+  const DictCounters c0{H.n_groups, 0u, H.arena_used, H.key_bytes_total};
+  CK(cudaMemcpy(&ctl()->dict, &c0, sizeof c0, cudaMemcpyHostToDevice));
   CK(launch_dict_restore(dict_view(), H.n_groups, stream)); stats.total_launches++;      // sets null_gid for the NULL-key group
   need_nullrows = (H.flags & 2) != 0; need_fz = (H.flags & 4) != 0;
   for (int64_t i = 0; i < H.n_panes; i++) {
@@ -1852,138 +1080,20 @@ void dnz_window::restore(const char* blob, size_t bytes) {
   fetch_ctl();
 }
 
-// ------------------------------------------------------------------------------------------------
-// pane exchange (see include/dnz_gpu.h)
-void dnz_window::export_partials(int64_t watermark, dnz_partials* out) {
-  process_pending(); drain();
-  memset(out, 0, sizeof *out);
-  h_owner_counts.assign((size_t)world, 0); h_owner_bytes.assign((size_t)world, 0);
-  out->owner_counts = h_owner_counts.data(); out->owner_key_bytes = h_owner_bytes.data();
-  out->pane_lo = 0; out->pane_hi = -1;
-  if (watermark == INT64_MIN) return;
-  const int64_t hi = floor_div(watermark, pane_ms) - 1;          // panes with end <= watermark
-  int64_t lo = exported_pane_upto == INT64_MIN ? (panes.empty() ? hi + 1 : panes.begin()->first) : exported_pane_upto + 1;
-  if (hi < lo) return;
-  std::vector<Pane*> send;
-  for (auto& kv : panes) if (kv.first >= lo && kv.first <= hi) send.push_back(kv.second.get());
-  out->pane_lo = lo; out->pane_hi = hi;
-  exported_pane_upto = hi;
-  if (send.empty()) return;
-  fetch_ctl();
-  if (n_groups_host == 0) return;
-  d_owner_cursor.reserve((size_t)world * 8);
-  h_small.reserve((size_t)std::max(256, world * 8));
-  PackParams P; memset(&P, 0, sizeof P);
-  P.n_groups = n_groups_host; P.rank = rank; P.world = world; P.dict = dict_view();
-  P.owner_cursor = d_owner_cursor.as<unsigned long long>();
-  auto run_pass = [&](int pass) {
-    CK(cudaMemsetAsync(d_owner_cursor.p, 0, (size_t)world * 8, stream));
-    P.pass = pass;
-    for (Pane* p : send) {
-      P.st = p->st.as<GroupState>(); P.nullrows = p->nullrows.as<unsigned long long>(); P.fz = p->fz.as<unsigned long long>(); P.pane = p->id;
-      CK(launch_pack_partials(P, stream)); stats.total_launches++;
-    }
-  };
-  run_pass(0);
-  CK(cudaMemcpyAsync(h_small.p, d_owner_cursor.p, (size_t)world * 8, cudaMemcpyDeviceToHost, stream));
-  CK(cudaStreamSynchronize(stream));
-  uint64_t n_total = 0, b_total = 0;
-  for (int o = 0; o < world; o++) {
-    uint64_t c = h_small.as<uint64_t>()[o];
-    h_owner_counts[(size_t)o] = (int64_t)(c >> 32); h_owner_bytes[(size_t)o] = (int64_t)(c & 0xFFFFFFFFull);
-    P.owner_base[o] = (n_total << 32) | b_total;
-    n_total += c >> 32; b_total += c & 0xFFFFFFFFull;
-    if (n_total >= (1ull << 31) || b_total >= (1ull << 31)) fail(DNZ_ERR_UNSUPPORTED, "more than 2^31 packets or key bytes in one exchange step");
-  }
-  if (n_total == 0) return;
-  d_part_entries.reserve((size_t)n_total * sizeof(PartialEntry)); d_part_keys.reserve((size_t)b_total + 64);
-  P.entries = d_part_entries.as<PartialEntry>(); P.key_bytes = d_part_keys.as<uint8_t>();
-  run_pass(1);
-  CK(cudaStreamSynchronize(stream));
-  out->n_entries = (int64_t)n_total; out->entries = d_part_entries.as<uint8_t>();
-  out->key_bytes_len = (int64_t)b_total; out->key_bytes = d_part_keys.as<uint8_t>();
-  stats.exchanged_out += (int64_t)n_total;
-}
-
-void dnz_window::import_partials(const uint8_t* entries, const int64_t* src_counts, const uint8_t* key_bytes,
-                                 const int64_t* src_key_bytes, int64_t pane_lo, int64_t pane_hi) {
-  MergeParams M; memset(&M, 0, sizeof M);
-  int64_t n = 0, kb = 0;
-  for (int r = 0; r < world; r++) {
-    if (src_counts[r] < 0 || src_key_bytes[r] < 0) fail(DNZ_ERR_INVALID, "negative split size");
-    M.src_key_base[r] = kb; n += src_counts[r]; kb += src_key_bytes[r]; M.src_entry_end[r] = n;
-  }
-  if (n == 0) return;
-  if (!entries || (kb && !key_bytes)) fail(DNZ_ERR_INVALID, "null packet buffers");
-  if (pane_hi < pane_lo || pane_hi - pane_lo >= (1 << 16)) fail(DNZ_ERR_INVALID, "bad pane range");
-  // every received key may be new here: size the dictionary and the long-key arena first so that the merge cannot fail
-  fetch_ctl();
-  while ((uint64_t)n_groups_host + (uint64_t)n > gcap) dict_grow();
-  {
-    if (arena_used_host + (uint64_t)kb + 64 > arena_cap) arena_grow(arena_used_host + (uint64_t)kb + 64);
-  }
-  const int64_t np = pane_hi - pane_lo + 1;
-  for (int64_t p = pane_lo; p <= pane_hi; p++) ensure_side_arrays(get_pane(p, true));
-  const size_t pb = (size_t)np * sizeof(void*);
-  h_xptrs.reserve(7 * pb); d_xptrs.reserve(7 * pb);
-  void** hp = h_xptrs.as<void*>();
-  for (int64_t p = pane_lo; p <= pane_hi; p++) {
-    const size_t k = (size_t)(p - pane_lo);
-    Pane* m = get_pane(p, false);
-    hp[0 * np + k] = m->st.p; hp[1 * np + k] = nullptr; hp[2 * np + k] = m->nullrows.p; hp[3 * np + k] = nullptr;
-    hp[4 * np + k] = m->fz.p; hp[5 * np + k] = nullptr; hp[6 * np + k] = reinterpret_cast<void*>((uintptr_t)(m->tag & 0xFFFFFFFFull));
-  }
-  CK(cudaMemcpyAsync(d_xptrs.p, hp, 7 * pb, cudaMemcpyHostToDevice, stream));
-  CK(cudaMemsetAsync(ctl(CTL_MERGE_ERR), 0, 4, stream));
-  char* dp = d_xptrs.as<char>();
-  M.panes.pane0 = pane_lo; M.panes.n_panes = (int32_t)np; M.panes.pane_ms = pane_ms;
-  M.panes.main = (GroupState* const*)(dp + 0 * pb); M.panes.late = (GroupState* const*)(dp + 1 * pb);
-  M.panes.nullrows_main = (unsigned long long* const*)(dp + 2 * pb); M.panes.nullrows_late = (unsigned long long* const*)(dp + 3 * pb);
-  M.panes.fz_main = (unsigned long long* const*)(dp + 4 * pb); M.panes.fz_late = (unsigned long long* const*)(dp + 5 * pb);
-  M.panes.tag_main = (const unsigned long long*)(dp + 6 * pb);
-  M.entries = reinterpret_cast<const PartialEntry*>(entries); M.n_entries = n; M.key_bytes = key_bytes; M.world = world;
-  M.dict = dict_view(); M.error = reinterpret_cast<uint32_t*>(ctl(CTL_MERGE_ERR));
-  CK(launch_merge_partials(M, stream)); stats.total_launches++;
-  fetch_ctl();
-  uint32_t err = *reinterpret_cast<const uint32_t*>(h_small.as<char>() + CTL_MERGE_ERR);
-  if (err) fail(DNZ_ERR_NOMEM, "pane merge failed (flags %u): table sizing error", err);
-  stats.exchanged_in += n;
-}
-
 // =================================================================================================
 // C ABI
 // =================================================================================================
-#define DNZ_TRY(w)                                                                  \
-  if (!(w)) { g_last_error = "null handle"; return DNZ_ERR_INVALID; }               \
-  if ((w)->sticky) return (w)->sticky;                                              \
-  cudaSetDevice((w)->dev);                                                          \
-  try {
-#define DNZ_CATCH(w)                                                                \
-  } catch (const DnzError& e) {                                                     \
-    (w)->err = e.msg; g_last_error = e.msg;                                         \
-    if (e.code == DNZ_ERR_CUDA || (w)->in_process) (w)->sticky = e.code;            \
-    return e.code;                                                                  \
-  } catch (const std::exception& e) {                                               \
-    (w)->err = e.what(); g_last_error = e.what(); return DNZ_ERR_NOMEM;             \
-  }                                                                                 \
-  return DNZ_OK;
-
 extern "C" {
 
 int32_t dnz_window_create(const dnz_window_config* cfg, const struct ArrowSchema* input_schema, dnz_window** out) {
   if (!out) { g_last_error = "null out"; return DNZ_ERR_INVALID; }
   *out = nullptr;
   dnz_window* w = nullptr;
-  try {
+  return create_guarded([&] {
     w = new dnz_window();
     w->init(cfg, input_schema);
     *out = w;
-    return DNZ_OK;
-  } catch (const DnzError& e) {
-    g_last_error = e.msg; delete w; return e.code;
-  } catch (const std::exception& e) {
-    g_last_error = e.what(); delete w; return DNZ_ERR_NOMEM;
-  }
+  }, [&] { delete w; });
 }
 
 int32_t dnz_window_push(dnz_window* w, struct ArrowArray* batch) {
@@ -2041,7 +1151,7 @@ int32_t dnz_window_flush(dnz_window* w, int64_t watermark_ms) {
   if (w->res_consumed) w->reset_results();
   w->rotate_result_sets();
   if (w->ungrouped) w->ungrouped_emit_run(nullptr, nullptr, nullptr, watermark_ms);
-  else w->emit_normal(watermark_ms, false, nullptr);
+  else w->emit_normal(watermark_ms, nullptr);
   DNZ_CATCH(w)
 }
 
@@ -2146,481 +1256,6 @@ int32_t dnz_memcpy(void* dst, const void* src, int64_t bytes, int32_t kind) {
   cudaError_t e = cudaMemcpy(dst, src, (size_t)bytes, kind == 1 ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost);
   if (e != cudaSuccess) { g_last_error = cudaGetErrorString(e); return DNZ_ERR_CUDA; }
   return DNZ_OK;
-}
-
-struct dnz_synth {
-  int dev; void* ts; void* val; void* off; void* bytes; int64_t alg_bytes;
-};
-
-int32_t dnz_synth_generate(int32_t device, int64_t row0, int64_t n_rows, int64_t batch_rows, uint64_t seed, int64_t groups,
-                           int64_t rows_per_ms, int64_t t0_ms, int32_t uuid_keys, int64_t key_mul, int64_t key_add, dnz_synth** arena,
-                           dnz_device_batch* out, int64_t n_batches) {
-  if (!arena || !out || n_rows <= 0 || batch_rows <= 0 || groups <= 0 || rows_per_ms <= 0) { g_last_error = "bad synth arguments"; return DNZ_ERR_INVALID; }
-  int64_t nb = (n_rows + batch_rows - 1) / batch_rows;
-  if (n_batches < nb) { g_last_error = "batch array too small"; return DNZ_ERR_INVALID; }
-  if (cudaSetDevice(device) != cudaSuccess) { g_last_error = "no such CUDA device"; return DNZ_ERR_CUDA; }
-  int maxlen = 36;
-  if (key_mul < 1) key_mul = 1;
-  if (!uuid_keys) { maxlen = 8; for (int64_t v = (groups - 1) * key_mul + key_add; v >= 10; v /= 10) maxlen++; }
-  int64_t off_stride = (batch_rows + 1 + 3) & ~(int64_t)3;
-  int64_t bytes_stride = (batch_rows * maxlen + 15 + 16) & ~(int64_t)15;
-  dnz_synth* a = new dnz_synth{device, nullptr, nullptr, nullptr, nullptr, 0};
-  auto bail = [&](const char* m) { g_last_error = m; dnz_synth_free(a); return DNZ_ERR_CUDA; };
-  if (cudaMalloc(&a->ts, (size_t)n_rows * 8 + 64) != cudaSuccess) return bail("cudaMalloc(ts) failed");
-  if (cudaMalloc(&a->val, (size_t)n_rows * 8 + 64) != cudaSuccess) return bail("cudaMalloc(val) failed");
-  if (cudaMalloc(&a->off, (size_t)nb * off_stride * 4 + 64) != cudaSuccess) return bail("cudaMalloc(off) failed");
-  if (cudaMalloc(&a->bytes, (size_t)nb * bytes_stride + 64) != cudaSuccess) return bail("cudaMalloc(bytes) failed");
-  if (launch_synth(row0, n_rows, batch_rows, seed, groups, rows_per_ms, t0_ms, uuid_keys, key_mul, key_add, (int64_t*)a->ts, (double*)a->val,
-                   (int32_t*)a->off, (uint8_t*)a->bytes, bytes_stride, nullptr) != cudaSuccess) return bail("synth launch failed");
-  if (cudaDeviceSynchronize() != cudaSuccess) return bail("synth kernel failed");
-  // algorithmic bytes: 20 B/row + key bytes (last offset of every batch)
-  std::vector<int32_t> last((size_t)nb);
-  for (int64_t b = 0; b < nb; b++) {
-    int64_t n = std::min(batch_rows, n_rows - b * batch_rows);
-    if (cudaMemcpy(&last[(size_t)b], (int32_t*)a->off + b * off_stride + n, 4, cudaMemcpyDeviceToHost) != cudaSuccess) return bail("memcpy failed");
-  }
-  a->alg_bytes = 20 * n_rows;
-  for (int64_t b = 0; b < nb; b++) {
-    int64_t n = std::min(batch_rows, n_rows - b * batch_rows);
-    a->alg_bytes += last[(size_t)b];
-    dnz_device_batch& d = out[b];
-    memset(&d, 0, sizeof d);
-    d.n_rows = n; d.ts = (int64_t*)a->ts + b * batch_rows; d.val = (double*)a->val + b * batch_rows;
-    d.key_off = (int32_t*)a->off + b * off_stride; d.key_bytes = (uint8_t*)a->bytes + b * bytes_stride;
-  }
-  *arena = a;
-  return DNZ_OK;
-}
-int64_t dnz_synth_bytes(const dnz_synth* a) { return a ? a->alg_bytes : 0; }
-void dnz_synth_free(dnz_synth* a) {
-  if (!a) return;
-  cudaSetDevice(a->dev);
-  cudaFree(a->ts); cudaFree(a->val); cudaFree(a->off); cudaFree(a->bytes);
-  delete a;
-}
-
-}  // extern "C"
-
-// =================================================================================================
-// dnz_group: the library-owned communicator of the fused pane exchange (SURVEY.md §8b "dnz_group_create"; §8e).
-// One rank per GPU.  Multi-process groups (one process per GPU, the production shape) map every rank's receive region into every
-// peer with CUDA IPC, order the streams of different ranks with INTERPROCESS CUDA EVENTS (no kernel ever spins) and exchange the
-// per-step host scalars (local watermark, first pane) through a POSIX shared-memory block; the rendezvous needs two all-gathers
-// of a few hundred bytes at creation, which the host application supplies as a callback (the role the ncclUniqueId broadcast
-// plays for NCCL).  Local groups put all ranks into one process (tests; several GPUs driven by one process): same kernels,
-// same protocol, plain events.
-// =================================================================================================
-#include <fcntl.h>
-#include <sys/mman.h>
-#include <unistd.h>
-
-#include <atomic>
-
-namespace {
-struct HostCtl {          // shared by all ranks (POSIX shm or heap); four slots by step & 3: a rank is never more than two steps ahead
-  std::atomic<int64_t> arrived[4][MAX_WORLD];     // phase 1: the local watermark of the step is published
-  std::atomic<int64_t> packed[4][MAX_WORLD];      // phase 2: the "my packets are written" event of the step is recorded
-  std::atomic<int64_t> finished[4][MAX_WORLD];    // phase 3: the step is issued completely ("merged" event recorded)
-  std::atomic<int64_t> lwm[4][MAX_WORLD];
-  std::atomic<int64_t> first_pane[4][MAX_WORLD];
-  std::atomic<int32_t> failed;
-};
-struct GroupShared { HostCtl ctl; };
-}  // namespace
-
-struct dnz_group {
-  int rank = 0, world = 1, dev = 0;
-  uint64_t ring_entries = 0, ring_key_bytes = 0;
-  size_t region_bytes = 0;
-  void* region = nullptr;                       // this rank's receive region (cudaMalloc: IPC-exportable)
-  std::vector<void*> peer_base;                 // mapped peers (nullptr for self)
-  bool ipc = false;
-  HostCtl* hctl = nullptr; size_t shm_bytes = 0; std::string shm_name; bool shm_owner = false;
-  std::shared_ptr<GroupShared> local_shared;
-  // ev_packed[r][p] / ev_merged[r][p]: rank r's events of step parity p (own rank: created here; peers: opened / shared)
-  cudaEvent_t ev_packed[MAX_WORLD][2] = {}, ev_merged[MAX_WORLD][2] = {};
-  XchgView view{};
-  unsigned long long step = 0;
-  DevBuf d_owner_cursor, d_owner_base, d_totals;   // totals: [0] packets sent, [1] packets merged
-  PinnedBuf h_totals; cudaEvent_t totals_ev = nullptr; bool totals_issued = false;
-  int phase = 0;                                 // 0 idle, 1 begun, 2 packed
-  // DNZ_TRACE: device timestamps of the step phases (pack start, packed, peers' packets seen, merged, emitted)
-  static constexpr int TSTEPS = 48; cudaEvent_t tev[TSTEPS][5] = {}; int tcount = 0;
-  void tmark(int k, cudaStream_t st) { if (!g_trace || tcount >= TSTEPS) return; if (!tev[tcount][k]) cudaEventCreate(&tev[tcount][k]); cudaEventRecord(tev[tcount][k], st); if (k == 4) tcount++; }
-  struct Range { int64_t gwm = INT64_MIN, first = INT64_MAX, hi = INT64_MIN; bool any = false; };
-  Range sent[2];                                 // what pack of step s sent (by step parity): merged by finish of step s+1
-  bool staged[2] = {false, false};
-  unsigned long long attach_step = 0;            // the step count when the current STREAM began (first step of a fresh operator): what was published before belongs to another stream
-
-  static XchgRegion carve(void* base, uint64_t ring_entries) {
-    XchgRegion r;
-    char* p = static_cast<char*>(base);
-    r.ctl = reinterpret_cast<XchgCtl*>(p);
-    r.entries = reinterpret_cast<PartialEntry*>(p + 4096);
-    r.keys = reinterpret_cast<uint8_t*>(p + 4096 + 2 * ring_entries * sizeof(PartialEntry));
-    return r;
-  }
-  ~dnz_group() {
-    cudaSetDevice(dev);
-    cudaDeviceSynchronize();
-    if (g_trace) for (int i = 0; i < tcount; i++) {
-      float a = 0, b = 0, c = 0, d = 0, gap = 0;
-      cudaEventElapsedTime(&a, tev[i][0], tev[i][1]); cudaEventElapsedTime(&b, tev[i][1], tev[i][2]); cudaEventElapsedTime(&c, tev[i][2], tev[i][3]); cudaEventElapsedTime(&d, tev[i][3], tev[i][4]);
-      if (i) cudaEventElapsedTime(&gap, tev[i - 1][4], tev[i][0]);
-      fprintf(stderr, "[dnz] rank %d xstep %d device: since_prev=%.3f pack=%.3f wait_peers=%.3f merge=%.3f emit=%.3f ms\n", rank, i, gap, a, b, c, d);
-    }
-    if (totals_ev) cudaEventDestroy(totals_ev);
-    for (int p = 0; p < 2; p++) { if (ev_packed[rank][p]) cudaEventDestroy(ev_packed[rank][p]); if (ev_merged[rank][p]) cudaEventDestroy(ev_merged[rank][p]); }
-    if (ipc) {
-      for (int r = 0; r < world; r++) if (r != rank) for (int p = 0; p < 2; p++) { if (ev_packed[r][p]) cudaEventDestroy(ev_packed[r][p]); if (ev_merged[r][p]) cudaEventDestroy(ev_merged[r][p]); }
-      for (size_t r = 0; r < peer_base.size(); r++) if (peer_base[r]) cudaIpcCloseMemHandle(peer_base[r]);
-    }
-    if (region) cudaFree(region);
-    if (hctl && !local_shared) { munmap(hctl, shm_bytes); if (shm_owner) shm_unlink(shm_name.c_str()); }
-  }
-};
-
-namespace {
-
-void group_alloc_region(dnz_group* g, unsigned event_flags) {
-  if (g->ring_entries < 1024) g->ring_entries = 1024;
-  if (g->ring_key_bytes < 65536) g->ring_key_bytes = 65536;
-  g->ring_key_bytes = round_up(g->ring_key_bytes, 256);
-  if (g->ring_entries >= (1ull << 31) || g->ring_key_bytes >= (1ull << 31)) fail(DNZ_ERR_INVALID, "exchange ring larger than 2^31 packets / key bytes per step");
-  g->region_bytes = 4096 + 2 * g->ring_entries * sizeof(PartialEntry) + 2 * g->ring_key_bytes;
-  CK(cudaSetDevice(g->dev));
-  CK(cudaMalloc(&g->region, g->region_bytes));
-  CK(cudaMemset(g->region, 0, 4096));
-  g->d_owner_cursor.alloc(MAX_WORLD * 8); g->d_owner_base.alloc(MAX_WORLD * 8); g->d_totals.alloc(64);
-  CK(cudaMemset(g->d_totals.p, 0, 64));
-  g->h_totals.reserve(64); memset(g->h_totals.p, 0, 64);
-  CK(cudaEventCreateWithFlags(&g->totals_ev, cudaEventDisableTiming));
-  for (int p = 0; p < 2; p++) {
-    CK(cudaEventCreateWithFlags(&g->ev_packed[g->rank][p], cudaEventDisableTiming | event_flags));
-    CK(cudaEventCreateWithFlags(&g->ev_merged[g->rank][p], cudaEventDisableTiming | event_flags));
-  }
-  CK(cudaDeviceSynchronize());
-}
-
-void group_finish_view(dnz_group* g) {
-  XchgView& v = g->view;
-  memset(&v, 0, sizeof v);
-  v.rank = g->rank; v.world = g->world; v.ring_entries = g->ring_entries; v.ring_key_bytes = g->ring_key_bytes;
-  v.self = dnz_group::carve(g->region, g->ring_entries);
-  for (int r = 0; r < g->world; r++) v.peer[r] = dnz_group::carve(r == g->rank ? g->region : g->peer_base[(size_t)r], g->ring_entries);
-}
-
-// host barrier on one of the per-step counters.  A process that drives all ranks itself must call the phases in order for
-// ALL ranks (begin x world, pack x world, finish x world): waiting would never end there, so it is an error instead.
-void group_wait(dnz_group* g, std::atomic<int64_t> (*ctr)[MAX_WORLD], unsigned long long step, const char* what) {
-  const int s = (int)(step & 3);
-  const auto t0 = std::chrono::steady_clock::now();
-  for (int r = 0; r < g->world; r++) {
-    int spins = 0;
-    while (ctr[s][r].load(std::memory_order_acquire) != (int64_t)step) {
-      if (g->local_shared) fail(DNZ_ERR_INVALID, "exchange group: rank %d has not reached '%s' of step %llu (a process driving several ranks calls each phase for all ranks before the next phase)", r, what, step);
-      if (g->hctl->failed.load(std::memory_order_relaxed)) fail(DNZ_ERR_INVALID, "exchange group: another rank failed or left");
-      if (++spins > 2000) {
-        usleep(50);
-        if (std::chrono::steady_clock::now() - t0 > std::chrono::seconds(300)) fail(DNZ_ERR_INVALID, "exchange group: rank %d did not reach '%s' of step %llu within 300 s", r, what, step);
-      }
-    }
-  }
-}
-
-}  // namespace
-
-// The step protocol is PIPELINED over three steps so that no phase waits for something a peer does "now" (a rank whose host
-// thread is descheduled for a millisecond would otherwise idle every GPU of the group -- each has about one aggregate launch
-// queued):
-//     step s   begin   publish this rank's local watermark                                        -> lwm(s)
-//     step s+1 pack    global watermark = min over ranks of lwm(s); the panes it closes are packed and written into the owners'
-//                      rings (half (s+1) & 1)
-//     step s+2 finish  the owners merge what step s+1 wrote, and emit the windows closed under that watermark
-// The only host wait is "every rank has ISSUED step s-1" (finished[s-1]), checked in pack of step s: it orders the interprocess
-// event waits (an event wait captures the record that exists when it is issued) and was normally satisfied a whole step ago.
-// Every rank computes the same watermark / pane range sequence, so `exported_pane_upto` agrees everywhere without being exchanged.
-
-// ---- phase 1: seal what is filling, publish the local watermark of the step
-void dnz_window::group_begin(dnz_group* g) {
-  if (world != g->world || rank != g->rank) fail(DNZ_ERR_INVALID, "operator is not attached to this group");
-  if (g->phase != 0) fail(DNZ_ERR_INVALID, "dnz_group_step_begin: the previous step of this rank is not finished");
-  // Nothing is waited for.  A filling superbatch is sealed (its scan is enqueued, the superbatch sealed before it is launched: its
-  // scan results are on the host), but the NEWEST sealed superbatch is not forced -- its scan sits behind the previous aggregate
-  // on the device, waiting for it here would idle the GPU every step.  The local watermark is that of the LAUNCHED batches;
-  // dnz_window_process before the step includes everything pushed.
-  // Errors of earlier steps (ring / table overflow) surface when their launches are verified.
-  if (!group_started) {
-    // The first step of a fresh operator begins a new stream in the group (collective: every rank's operator is fresh in the same
-    // step; operators may have been attached long before).  Watermarks published and pane ranges sent before this step belong to
-    // the previous stream: the pipeline restarts empty.
-    group_started = true;
-    g->attach_step = g->step; g->sent[0] = g->sent[1] = dnz_group::Range{};
-  }
-  if (!cur().batches.empty()) seal_current();
-  while (!launched_order.empty() && cudaEventQuery(slot[launched_order.front()].done) == cudaSuccess) verify(slot[launched_order.front()]);
-  cudaGetLastError();
-  if (g->totals_issued && cudaEventQuery(g->totals_ev) == cudaSuccess) {
-    stats.exchanged_out = (int64_t)g->h_totals.as<unsigned long long>()[0]; stats.exchanged_in = (int64_t)g->h_totals.as<unsigned long long>()[1];
-  }
-  cudaGetLastError();
-  const unsigned long long step = g->step + 1;
-  HostCtl* h = g->hctl; const int q = (int)(step & 3);
-  h->lwm[q][g->rank].store(has_lwm ? lwm : INT64_MIN, std::memory_order_relaxed);
-  h->first_pane[q][g->rank].store(panes.empty() ? INT64_MAX : panes.begin()->first, std::memory_order_relaxed);
-  h->arrived[q][g->rank].store((int64_t)step, std::memory_order_release);
-  g->phase = 1;
-  g_tr.mark("x_begin");
-}
-
-// ---- phase 2: the panes closed under the watermark published one step ago go straight into the owners' rings
-void dnz_window::group_pack(dnz_group* g) {
-  if (g->phase != 1) fail(DNZ_ERR_INVALID, "dnz_group_step_pack without dnz_group_step_begin");
-  const unsigned long long step = g->step + 1;
-  const int par = (int)(step & 1);
-  int64_t gwm = INT64_MIN, gfirst = INT64_MAX;
-  if (step >= 2) {
-    group_wait(g, g->hctl->finished, step - 1, "finish");
-    g_tr.mark("x_wait_prev_step");
-    const int q = (int)((step - 1) & 3);
-    if (step - 1 > g->attach_step) gwm = INT64_MAX;          // (the watermarks of step-1 were published by THIS stream's operators)
-    if (step - 1 > g->attach_step) for (int r = 0; r < world; r++) { gwm = std::min(gwm, g->hctl->lwm[q][r].load(std::memory_order_relaxed)); gfirst = std::min(gfirst, g->hctl->first_pane[q][r].load(std::memory_order_relaxed)); }
-  }
-  if (exported_pane_upto != INT64_MIN) gfirst = exported_pane_upto + 1;
-  const int64_t hi = gwm == INT64_MIN ? INT64_MIN : floor_div(gwm, pane_ms) - 1;          // panes with end <= global watermark
-  const bool any = gwm != INT64_MIN && gfirst != INT64_MAX && hi >= gfirst;
-  g->sent[par].gwm = gwm; g->sent[par].first = gfirst; g->sent[par].hi = hi; g->sent[par].any = any;
-  XchgView X = g->view; X.step = step;
-  std::vector<Pane*> send;
-  if (any) {
-    if (hi - gfirst + 1 > (1 << 16)) fail(DNZ_ERR_UNSUPPORTED, "one exchange step spans %lld panes", (long long)(hi - gfirst + 1));
-    for (auto& kv : panes) if (kv.first >= gfirst && kv.first <= hi) send.push_back(kv.second.get());
-    exported_pane_upto = hi;                                                                // the same on every rank
-  }
-  // the owners must have merged what step-2 wrote into the same half of their rings (recorded in their finish of step-1)
-  if (step > 2) for (int r = 0; r < world; r++) if (r != rank) CK(cudaStreamWaitEvent(stream, g->ev_merged[r][par], 0));
-  g->tmark(0, stream);
-  CK(cudaMemsetAsync(g->d_owner_cursor.p, 0, MAX_WORLD * 8, stream));
-  PackParams P; memset(&P, 0, sizeof P);
-  P.n_groups = gcap; P.rank = rank; P.world = world; P.dict = dict_view();      // grid bound; the kernels clamp to the device counter
-  P.owner_cursor = g->d_owner_cursor.as<unsigned long long>();
-  auto for_pane_chunks = [&](auto&& launch) {                 // up to PACK_PANES panes per launch (one thread per group id walks them)
-    for (size_t i0 = 0; i0 < send.size(); i0 += PACK_PANES) {
-      P.n_multi = (int32_t)std::min<size_t>(PACK_PANES, send.size() - i0);
-      for (int j = 0; j < P.n_multi; j++) {
-        Pane* p = send[i0 + j];
-        P.mst[j] = p->st.as<GroupState>(); P.mnull[j] = p->nullrows.as<unsigned long long>(); P.mfz[j] = p->fz.as<unsigned long long>(); P.mpane[j] = p->id;
-      }
-      launch(); stats.total_launches++;
-    }
-  };
-  P.pass = 0;
-  for_pane_chunks([&]() { CK(launch_pack_partials(P, stream)); });
-  CK(launch_xchg_reserve(X, g->d_owner_cursor.as<unsigned long long>(), g->d_owner_base.as<unsigned long long>(), g->d_totals.as<unsigned long long>(), reinterpret_cast<uint32_t*>(ctl(CTL_MERGE_ERR)), stream));
-  stats.total_launches++;
-  for_pane_chunks([&]() { CK(launch_pack_write_peer(P, X, g->d_owner_base.as<unsigned long long>(), stream)); });
-  CK(cudaEventRecord(g->ev_packed[rank][par], stream));                    // "all my packets of this step are in the owners' rings"
-  g->tmark(1, stream);
-  g->hctl->packed[(int)(step & 3)][g->rank].store((int64_t)step, std::memory_order_release);
-  g->phase = 2;
-  g_tr.mark("x_pack");
-}
-
-// ---- phase 3: merge what the peers wrote ONE STEP AGO, emit the windows of this rank's keys closed under that step's watermark
-void dnz_window::group_finish(dnz_group* g, int64_t* gwm_out) {
-  if (g->phase != 2) fail(DNZ_ERR_INVALID, "dnz_group_step_finish without dnz_group_step_pack");
-  const unsigned long long step = ++g->step;
-  g->phase = 0;
-  if (gwm_out) *gwm_out = INT64_MIN;
-  if (step >= 2) {
-    const unsigned long long mstep = step - 1;                            // the step whose packets are merged now
-    const int mp = (int)(mstep & 1);
-    const dnz_group::Range R = g->sent[mp];
-    if (gwm_out) *gwm_out = R.gwm;
-    XchgView X = g->view; X.step = mstep;
-    // every peer issued pack(mstep) before its finish(mstep), which pack of this step waited for: the records exist
-    for (int r = 0; r < world; r++) if (r != rank) CK(cudaStreamWaitEvent(stream, g->ev_packed[r][mp], 0));
-    g->tmark(2, stream);
-    if (R.any) {
-      const int64_t gfirst = R.first, hi = R.hi;
-      const int64_t np = hi - gfirst + 1;
-      for (int64_t p = gfirst; p <= hi; p++) ensure_side_arrays(get_pane(p, true));
-      const size_t pb = (size_t)np * sizeof(void*);
-      // The pane table is staged in page-locked memory and copied by the stream when it gets there: the staging half may only be
-      // rewritten once the copy issued two steps ago (same half) has executed -- its merge has been recorded in ev_merged[rank][mp].
-      const size_t half_bytes = (size_t)7 * (1 << 16) * sizeof(void*);
-      if (g->staged[mp]) CK(cudaEventSynchronize(g->ev_merged[rank][mp]));
-      g->staged[mp] = true;
-      g_tr.mark("x_sync_merged");
-      void** hp = reinterpret_cast<void**>(h_xptrs.as<char>() + (size_t)mp * half_bytes);
-      char* dxp = d_xptrs.as<char>() + (size_t)mp * half_bytes;
-      for (int64_t p = gfirst; p <= hi; p++) {
-        const size_t k = (size_t)(p - gfirst);
-        Pane* m = get_pane(p, false);
-        hp[0 * np + k] = m->st.p; hp[1 * np + k] = nullptr; hp[2 * np + k] = m->nullrows.p; hp[3 * np + k] = nullptr;
-        hp[4 * np + k] = m->fz.p; hp[5 * np + k] = nullptr; hp[6 * np + k] = reinterpret_cast<void*>((uintptr_t)(m->tag & 0xFFFFFFFFull));
-      }
-      CK(cudaMemcpyAsync(dxp, hp, 7 * pb, cudaMemcpyHostToDevice, stream));
-      MergeParams M; memset(&M, 0, sizeof M);
-      char* dp = dxp;
-      M.panes.pane0 = gfirst; M.panes.n_panes = (int32_t)np; M.panes.pane_ms = pane_ms;
-      M.panes.main = (GroupState* const*)(dp + 0 * pb); M.panes.late = (GroupState* const*)(dp + 1 * pb);
-      M.panes.nullrows_main = (unsigned long long* const*)(dp + 2 * pb); M.panes.nullrows_late = (unsigned long long* const*)(dp + 3 * pb);
-      M.panes.fz_main = (unsigned long long* const*)(dp + 4 * pb); M.panes.fz_late = (unsigned long long* const*)(dp + 5 * pb);
-      M.panes.tag_main = (const unsigned long long*)(dp + 6 * pb);
-      M.world = world; M.dict = dict_view(); M.error = reinterpret_cast<uint32_t*>(ctl(CTL_MERGE_ERR));
-      CK(launch_merge_ring(M, X, g->d_totals.as<unsigned long long>() + 1, sm_count, stream)); stats.total_launches++;
-    }
-    CK(cudaMemsetAsync(&g->view.self.ctl->cursor[mp], 0, 8, stream));       // the ring half is free again ...
-    CK(cudaEventRecord(g->ev_merged[rank][mp], stream));                    // ... once this has happened
-    CK(cudaMemcpyAsync(g->h_totals.p, g->d_totals.p, 16, cudaMemcpyDeviceToHost, stream));   // packet counters for dnz_stats (read when complete)
-    CK(cudaEventRecord(g->totals_ev, stream)); g->totals_issued = true;
-    g->tmark(3, stream);
-    // ---- every rank emits the windows of ITS keys that closed under that watermark
-    if (R.gwm != INT64_MIN) {
-      if (res_consumed) reset_results();
-      rotate_result_sets();
-      emit_normal(R.gwm, false, nullptr);
-    }
-    g->tmark(4, stream);
-  }
-  g->hctl->finished[(int)(step & 3)][g->rank].store((int64_t)step, std::memory_order_release);
-  g_tr.mark("x_finish");
-  g_tr.flush("xstep");
-}
-
-namespace {
-struct GroupHello { cudaIpcMemHandle_t mem; cudaIpcEventHandle_t packed[2], merged[2]; char shm[64]; int64_t ring_entries, ring_key_bytes; int32_t dev, pad; };
-}
-
-extern "C" {
-
-int32_t dnz_group_create(const dnz_group_config* cfg, dnz_allgather_fn allgather, void* ctx, dnz_group** out) {
-  if (!out) { g_last_error = "null out"; return DNZ_ERR_INVALID; }
-  *out = nullptr;
-  dnz_group* g = nullptr;
-  try {
-    if (!cfg || !allgather) fail(DNZ_ERR_INVALID, "null config or all-gather callback");
-    if (cfg->abi_version != DNZ_ABI_VERSION) fail(DNZ_ERR_INVALID, "abi_version %u != %u", cfg->abi_version, DNZ_ABI_VERSION);
-    if (cfg->world < 1 || cfg->world > MAX_WORLD || cfg->rank < 0 || cfg->rank >= cfg->world) fail(DNZ_ERR_INVALID, "bad rank/world (world <= %d)", MAX_WORLD);
-    g = new dnz_group();
-    g->rank = cfg->rank; g->world = cfg->world; g->dev = cfg->device; g->ipc = true;
-    g->ring_entries = (uint64_t)std::max<int64_t>(cfg->ring_entries, 0); g->ring_key_bytes = (uint64_t)std::max<int64_t>(cfg->ring_key_bytes, 0);
-    if (!g->ring_entries) g->ring_entries = 8ull << 20;
-    if (!g->ring_key_bytes) g->ring_key_bytes = 256ull << 20;
-    group_alloc_region(g, cudaEventInterprocess);
-    GroupHello mine; memset(&mine, 0, sizeof mine);
-    CK(cudaIpcGetMemHandle(&mine.mem, g->region));
-    for (int p = 0; p < 2; p++) { CK(cudaIpcGetEventHandle(&mine.packed[p], g->ev_packed[g->rank][p])); CK(cudaIpcGetEventHandle(&mine.merged[p], g->ev_merged[g->rank][p])); }
-    mine.ring_entries = (int64_t)g->ring_entries; mine.ring_key_bytes = (int64_t)g->ring_key_bytes; mine.dev = g->dev;
-    g->shm_bytes = round_up(sizeof(HostCtl), 4096);
-    if (g->rank == 0) {       // the block of per-step scalars shared by all ranks
-      snprintf(mine.shm, sizeof mine.shm, "/dnz_group_%d_%lld", (int)getpid(), (long long)std::chrono::steady_clock::now().time_since_epoch().count());
-      int fd = shm_open(mine.shm, O_CREAT | O_EXCL | O_RDWR, 0600);
-      if (fd < 0 || ftruncate(fd, (off_t)g->shm_bytes) != 0) fail(DNZ_ERR_NOMEM, "shm_open(%s) failed", mine.shm);
-      void* p = mmap(nullptr, g->shm_bytes, PROT_READ | PROT_WRITE, MAP_SHARED, fd, 0); close(fd);
-      if (p == MAP_FAILED) fail(DNZ_ERR_NOMEM, "mmap of the group control block failed");
-      g->hctl = static_cast<HostCtl*>(p); g->shm_name = mine.shm; g->shm_owner = true;
-    }
-    std::vector<GroupHello> all((size_t)g->world);
-    if (allgather(ctx, &mine, all.data(), (int64_t)sizeof(GroupHello)) != 0) fail(DNZ_ERR_INVALID, "the rendezvous all-gather failed");
-    if (g->rank != 0) {
-      int fd = shm_open(all[0].shm, O_RDWR, 0600);
-      if (fd < 0) fail(DNZ_ERR_INVALID, "cannot open the group control block %s (ranks must share one node)", all[0].shm);
-      void* p = mmap(nullptr, g->shm_bytes, PROT_READ | PROT_WRITE, MAP_SHARED, fd, 0); close(fd);
-      if (p == MAP_FAILED) fail(DNZ_ERR_NOMEM, "mmap of the group control block failed");
-      g->hctl = static_cast<HostCtl*>(p); g->shm_name = all[0].shm;
-    }
-    g->peer_base.assign((size_t)g->world, nullptr);
-    for (int r = 0; r < g->world; r++) {
-      const GroupHello& o = all[(size_t)r];
-      if (o.ring_entries != mine.ring_entries || o.ring_key_bytes != mine.ring_key_bytes) fail(DNZ_ERR_INVALID, "ranks disagree on the ring size");
-      if (r == g->rank) continue;
-      int can = 0; CK(cudaDeviceCanAccessPeer(&can, g->dev, o.dev));
-      if (!can && o.dev != g->dev) fail(DNZ_ERR_UNSUPPORTED, "GPU %d cannot access GPU %d directly (the fused exchange needs NVLink / P2P)", g->dev, o.dev);
-      CK(cudaIpcOpenMemHandle(&g->peer_base[(size_t)r], o.mem, cudaIpcMemLazyEnablePeerAccess));
-      for (int p = 0; p < 2; p++) { CK(cudaIpcOpenEventHandle(&g->ev_packed[r][p], o.packed[p])); CK(cudaIpcOpenEventHandle(&g->ev_merged[r][p], o.merged[p])); }
-    }
-    group_finish_view(g);
-    GroupHello again = mine; std::vector<GroupHello> all2((size_t)g->world);          // barrier: everybody has mapped everything
-    if (allgather(ctx, &again, all2.data(), (int64_t)sizeof(GroupHello)) != 0) fail(DNZ_ERR_INVALID, "the rendezvous all-gather failed");
-    if (g->shm_owner) { shm_unlink(g->shm_name.c_str()); g->shm_owner = false; }      // the mappings stay; the name is gone
-    *out = g;
-    return DNZ_OK;
-  } catch (const DnzError& e) {
-    g_last_error = e.msg; delete g; return e.code;
-  } catch (const std::exception& e) {
-    g_last_error = e.what(); delete g; return DNZ_ERR_NOMEM;
-  }
-}
-
-int32_t dnz_group_create_local(int32_t world, const int32_t* devices, int64_t ring_entries, int64_t ring_key_bytes, dnz_group** out) {
-  if (!out || !devices) { g_last_error = "null argument"; return DNZ_ERR_INVALID; }
-  std::vector<dnz_group*> gs;
-  try {
-    if (world < 1 || world > MAX_WORLD) fail(DNZ_ERR_INVALID, "bad world (<= %d)", MAX_WORLD);
-    auto shared = std::make_shared<GroupShared>();
-    memset(static_cast<void*>(&shared->ctl), 0, sizeof(HostCtl));
-    for (int r = 0; r < world; r++) {
-      dnz_group* g = new dnz_group(); gs.push_back(g);
-      g->rank = r; g->world = world; g->dev = devices[r];
-      g->ring_entries = ring_entries > 0 ? (uint64_t)ring_entries : (1ull << 20); g->ring_key_bytes = ring_key_bytes > 0 ? (uint64_t)ring_key_bytes : (32ull << 20);
-      g->local_shared = shared; g->hctl = &shared->ctl;
-      group_alloc_region(g, 0);
-    }
-    for (int r = 0; r < world; r++) {
-      dnz_group* g = gs[(size_t)r];
-      g->peer_base.assign((size_t)world, nullptr);
-      for (int q = 0; q < world; q++) {
-        if (q == r) continue;
-        g->peer_base[(size_t)q] = gs[(size_t)q]->region;
-        for (int p = 0; p < 2; p++) { g->ev_packed[q][p] = gs[(size_t)q]->ev_packed[q][p]; g->ev_merged[q][p] = gs[(size_t)q]->ev_merged[q][p]; }
-        if (devices[q] != devices[r]) { CK(cudaSetDevice(devices[r])); cudaError_t e = cudaDeviceEnablePeerAccess(devices[q], 0); if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CK(e); cudaGetLastError(); }
-      }
-      group_finish_view(g);
-    }
-    for (int r = 0; r < world; r++) out[r] = gs[(size_t)r];
-    return DNZ_OK;
-  } catch (const DnzError& e) {
-    g_last_error = e.msg; for (auto* g : gs) delete g; return e.code;
-  } catch (const std::exception& e) {
-    g_last_error = e.what(); for (auto* g : gs) delete g; return DNZ_ERR_NOMEM;
-  }
-}
-
-void dnz_group_destroy(dnz_group* g) {
-  if (!g) return;
-  if (g->hctl && !g->local_shared) g->hctl->failed.store(1);
-  delete g;
-}
-
-int32_t dnz_group_attach(dnz_group* g, dnz_window* w) {
-  if (!g) { g_last_error = "null group"; return DNZ_ERR_INVALID; }
-  const int32_t rc = dnz_window_set_exchange(w, g->rank, g->world);
-  if (rc == DNZ_OK) w->fused = g->world > 1;
-  return rc;
-}
-
-#define DNZ_GROUP_PHASE(call)                                                       \
-  DNZ_TRY(w)                                                                        \
-  if (!g) fail(DNZ_ERR_INVALID, "null group");                                      \
-  struct Guard { dnz_window* w; bool prev; ~Guard() { w->in_process = prev; } } guard{w, w->in_process};   \
-  w->in_process = true;                                                             \
-  call;                                                                             \
-  DNZ_CATCH(w)
-
-int32_t dnz_group_step_begin(dnz_group* g, dnz_window* w) { DNZ_GROUP_PHASE(w->group_begin(g)) }
-int32_t dnz_group_step_pack(dnz_group* g, dnz_window* w) { DNZ_GROUP_PHASE(w->group_pack(g)) }
-int32_t dnz_group_step_finish(dnz_group* g, dnz_window* w, int64_t* global_watermark_ms) { DNZ_GROUP_PHASE(w->group_finish(g, global_watermark_ms)) }
-int32_t dnz_group_step(dnz_group* g, dnz_window* w, int64_t* global_watermark_ms) {
-  int32_t rc = dnz_group_step_begin(g, w);
-  if (rc == DNZ_OK) rc = dnz_group_step_pack(g, w);
-  return rc != DNZ_OK ? rc : dnz_group_step_finish(g, w, global_watermark_ms);
-}
-int32_t dnz_group_flush(dnz_group* g, dnz_window* w, int64_t* global_watermark_ms) {
-  int32_t rc = dnz_window_process(w, nullptr);
-  for (int i = 0; i < 3 && rc == DNZ_OK; i++) rc = dnz_group_step(g, w, global_watermark_ms);
-  return rc;
 }
 
 }  // extern "C"
