@@ -1,5 +1,5 @@
 // dnz_device.cuh -- device helpers: PTX wrappers (mbarrier, cp.async.bulk, wide loads, reductions),
-// ordered float keys, key loading / hashing, dictionary probe+insert, per-row state update.
+// key loading / hashing, dictionary probe+insert, per-row state update, fold of partial states.
 #pragma once
 #include "dnz_kernels.h"
 
@@ -90,20 +90,6 @@ __device__ __forceinline__ void red_min_u64(unsigned long long* p, unsigned long
   asm volatile("red.global.min.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
-// ---------------------------------------------------------------- ordered float keys
-// ord(): monotone map f64 -> u64 over IEEE totalOrder.  min/max accumulators are kept as distances from the
-// DataFusion starting values (f64::MAX for min, f64::MIN for max) so that a zero-filled state IS the start.
-constexpr unsigned long long SIGN64 = 0x8000000000000000ull;
-constexpr unsigned long long BITS_F64_MAX = 0x7FEFFFFFFFFFFFFFull;
-constexpr unsigned long long ORD_F64_MAX = BITS_F64_MAX | SIGN64;        // ord(+MAX)
-constexpr unsigned long long ORD_F64_MIN = ~(BITS_F64_MAX | SIGN64);     // ord(-MAX)
-__host__ __device__ __forceinline__ unsigned long long ord_bits(unsigned long long b) { return (b & SIGN64) ? ~b : (b | SIGN64); }
-__host__ __device__ __forceinline__ unsigned long long unord_bits(unsigned long long o) { return (o & SIGN64) ? (o & ~SIGN64) : ~o; }
-// IEEE totalOrder key (arrow-ord cmp on floats == f64::total_cmp)
-__host__ __device__ __forceinline__ long long total_key(unsigned long long b) {
-  long long s = (long long)b; return s ^ (long long)(((unsigned long long)(s >> 63)) >> 1);
-}
-
 // ---------------------------------------------------------------- hashing
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
   x ^= x >> 32; x *= 0xD6E8FEB86659FD93ull; x ^= x >> 32; x *= 0xD6E8FEB86659FD93ull; x ^= x >> 32; return x;
@@ -121,6 +107,14 @@ __host__ __device__ __forceinline__ uint32_t hash_words(uint32_t w0, uint32_t w1
 }
 __host__ __device__ __forceinline__ uint64_t hash_inline(uint64_t k0, uint64_t k1, uint32_t len) {
   return hash_words((uint32_t)k0, (uint32_t)(k0 >> 32), (uint32_t)k1, (uint32_t)(k1 >> 32), len);
+}
+// hash of a key as DictSlot / GidKey hold it (a long key's k0 already is the hash of all its bytes)
+__host__ __device__ __forceinline__ uint64_t stored_key_hash(uint64_t k0, uint64_t k1, uint32_t len) {
+  return len <= (uint32_t)INLINE_KEY ? hash_inline(k0, k1, len) : k0;
+}
+// multi-GPU owner of a group: the rank that merges its partial states and emits it (the NULL key belongs to rank 0)
+__host__ __device__ __forceinline__ int key_owner(const GidKey& gk, int world) {
+  return gk.len == 0xFFFFFFFFu ? 0 : (int)(stored_key_hash(gk.k0, gk.k1, gk.len) % (uint64_t)world);
 }
 
 // A key as the dictionary sees it.
@@ -192,6 +186,25 @@ __device__ __forceinline__ uint8_t ld_key_byte(const uint8_t* p, bool shared) {
 // ---------------------------------------------------------------- dictionary
 enum : uint32_t { GID_DEFER_GROUPS = 0xFFFFFFFEu, GID_DEFER_ARENA = 0xFFFFFFFDu };
 
+// Publish a slot this thread has LOCKED: the key words with one 16 B store (what ld_slot's torn-read argument relies on), the
+// length, then the state with a release store.
+__device__ __forceinline__ void slot_publish(DictSlot* slot, uint64_t k0, uint64_t k1, uint32_t len, uint32_t state) {
+  st_relaxed_b128(&slot->k0, k0, k1);
+  slot->len = len;
+  __threadfence();
+  st_release_u32(&slot->state, state);
+}
+
+// Place a key that is not in the table yet (rehash, checkpoint restore): claim the first empty slot from `hash`, set its hint
+// before the publish.  Keys are never compared, so no two threads may place the same key.
+__device__ __forceinline__ void dict_place(const DictView& d, uint64_t hash, uint64_t k0, uint64_t k1, uint32_t len, uint64_t hint,
+                                           uint32_t state) {
+  uint32_t idx = (uint32_t)hash & d.mask;
+  while (atomicCAS(&d.slots[idx].state, SLOT_EMPTY, SLOT_LOCKED) != SLOT_EMPTY) idx = (idx + 1) & d.mask;
+  d.slots[idx].hint = hint;
+  slot_publish(d.slots + idx, k0, k1, len, state);
+}
+
 // Try to claim `slot` for key k.  Returns gid, or GID_DEFER_* when a table is full, or 0xFFFFFFFF when the CAS was
 // lost (caller re-examines the slot).
 __device__ __forceinline__ uint32_t dict_try_insert(const DictView& d, DictSlot* slot, uint32_t slot_idx, const KeyRef& k,
@@ -208,6 +221,8 @@ __device__ __forceinline__ uint32_t dict_try_insert(const DictView& d, DictSlot*
   // run past gcap; ids >= gcap are never used (the rows are deferred) and the host clamps the counter before it grows.
   uint32_t g = atomicAdd(d.n_groups, 1u);
   if (g >= d.gcap) { st_release_u32(&slot->state, SLOT_EMPTY); return GID_DEFER_GROUPS; }
+  // slot_publish's protocol, written out: k_aggregate's machine code is held as it is, with the gid_key store and the byte count
+  // between the length store and the fence
   if (k.len > (uint32_t)INLINE_KEY) {
     for (uint32_t i = 0; i < k.len; i++) d.arena[arena_off + i] = ld_key_byte(k.ptr + i, key_shared);
     st_relaxed_b128(&slot->k0, k.k0, arena_off);
@@ -296,8 +311,6 @@ __device__ __forceinline__ uint32_t dict_lookup(const DictView& d, const KeyRef&
 // DataFusion-42 semantics (SURVEY.md §8a-5): count += 1 per non-null value; min: `if cur > v`, max: `if cur < v`
 // from f64::MAX / f64::MIN (NaN never replaces, +inf never lowers min's start, -inf never raises max's start,
 // the first +-0.0 wins); avg = sum / count.
-__device__ __forceinline__ bool value_needs_fz(double v) { return v == 0.0; }
-
 __device__ __forceinline__ void state_update(GroupState* st, unsigned long long* fz, uint32_t gid, double v,
                                              unsigned long long rowseq) {
   GroupState* s = st + gid;
@@ -312,6 +325,18 @@ __device__ __forceinline__ void state_update(GroupState* st, unsigned long long*
   if (v <= 1.7976931348623157e308) red_max_u64(&s->minkey, ORD_F64_MAX - o);    // false for NaN and +inf
   if (v >= -1.7976931348623157e308) red_max_u64(&s->maxkey, o - ORD_F64_MIN);   // false for NaN and -inf
 }
+
+// Fold of partial states (per-CTA copies, warp partials, panes), added in the caller's order: counts add; the sum starts at the
+// first partial with a non-zero count, so that an empty partial never adds +0.0 to a -0.0 sum; minkey / maxkey take the max.
+// Count: double, or an exact integer where the caller keeps one.
+template <typename Count>
+struct StateFold {
+  Count cnt = 0; double sum = 0.0; unsigned long long mnk = 0, mxk = 0; bool first = true;
+  __device__ __forceinline__ void add(const GroupState& s) {
+    if (s.cnt != 0.0) { sum = first ? s.sum : sum + s.sum; first = false; }
+    cnt += (Count)s.cnt; mnk = max(mnk, s.minkey); mxk = max(mxk, s.maxkey);
+  }
+};
 
 __device__ __forceinline__ void defer_row(const DeferList& dl, uint32_t tile, uint32_t row, uint32_t why) {
   atomicOr(dl.flags, why);

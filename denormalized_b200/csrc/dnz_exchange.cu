@@ -26,23 +26,15 @@ __device__ __forceinline__ unsigned long long block_reserve(bool active, int own
   return active ? s_base[owner] + (((unsigned long long)lc << 32) | lb) : 0ull;
 }
 
-// ---- pack: thread per group id of one pane; two passes (count, then write) over every pane of the export ----------------
-// pane j of the launch (a launch covers up to PACK_PANES panes; n_multi == 0: the single pane in st / nullrows / fz / pane)
-struct PackPane { const GroupState* st; const unsigned long long* nu; const unsigned long long* fz; int64_t pane; };
-__device__ __forceinline__ PackPane pack_pane(const PackParams& P, int j) {
-  if (P.n_multi) return PackPane{P.mst[j], P.mnull[j], P.mfz[j], P.mpane[j]};
-  return PackPane{P.st, P.nullrows, P.fz, P.pane};
-}
+// ---- pack: thread per group id, up to PACK_PANES panes per launch; two passes (count, then write) over every pane sent ----
 // One thread per group id: which of the launch's panes hold something for it (bit mask), its key, its owner.
 struct PackCell { uint32_t amask; bool null_key; uint32_t klen, kpad; int owner; GidKey gk; };
 __device__ __forceinline__ PackCell pack_cell(const PackParams& P, uint32_t g) {
   PackCell c{}; c.amask = 0u;
   if (g >= P.n_groups || g >= min(*P.dict.n_groups, P.dict.gcap)) return c;    // n_groups may be an upper bound (fused path)
-  const int np = P.n_multi ? P.n_multi : 1;
-  for (int j = 0; j < np; j++) {
-    const PackPane pp = pack_pane(P, j);
-    const double cnt = pp.st[g].cnt;
-    const unsigned long long nr = pp.nu ? pp.nu[g] : 0ull;
+  for (int j = 0; j < P.n_panes; j++) {
+    const double cnt = P.st[j][g].cnt;
+    const unsigned long long nr = P.nullrows[j] ? P.nullrows[j][g] : 0ull;
     if (!(cnt == 0.0 && nr == 0ull)) c.amask |= 1u << j;
   }
   if (!c.amask) return c;
@@ -50,38 +42,48 @@ __device__ __forceinline__ PackCell pack_cell(const PackParams& P, uint32_t g) {
   c.null_key = c.gk.len == 0xFFFFFFFFu;
   c.klen = c.null_key ? 0u : c.gk.len;
   c.kpad = (c.klen + 7u) & ~7u;
-  c.owner = c.null_key ? 0 : (int)((c.klen <= (uint32_t)INLINE_KEY ? hash_inline(c.gk.k0, c.gk.k1, c.klen) : c.gk.k0) % (uint64_t)P.world);
+  c.owner = key_owner(c.gk, P.world);
   if (c.owner == P.rank) c.amask = 0u;
   return c;
 }
-__device__ __forceinline__ PartialEntry pack_entry(const PackPane& pp, uint32_t g, uint32_t key_off, const PackCell& c) {
-  const GroupState s = pp.st[g];
+__device__ __forceinline__ PartialEntry pack_entry(const PackParams& P, int j, uint32_t g, uint32_t key_off, const PackCell& c) {
+  const GroupState s = P.st[j][g];
   PartialEntry e;
-  e.pane = pp.pane; e.cnt = (unsigned long long)s.cnt; e.sum = s.sum; e.minkey = s.minkey; e.maxkey = s.maxkey;
-  e.nullrows = pp.nu ? pp.nu[g] : 0ull; e.fz = pp.fz ? pp.fz[g] : ~0ull;
+  e.pane = P.pane[j]; e.cnt = (unsigned long long)s.cnt; e.sum = s.sum; e.minkey = s.minkey; e.maxkey = s.maxkey;
+  e.nullrows = P.nullrows[j] ? P.nullrows[j][g] : 0ull; e.fz = P.fz[j] ? P.fz[j][g] : ~0ull;
   e.key_off = key_off; e.key_len = c.null_key ? 0xFFFFFFFFu : c.klen;
   return e;
 }
+// A 64 B packet leaves as four 128-bit stores, the widest store sm_90 has (a peer write travels NVLink per store instruction).
+__device__ __forceinline__ void store_packet(PartialEntry* dst, const PartialEntry& e) {
+  const unsigned long long* w = reinterpret_cast<const unsigned long long*>(&e);
+#pragma unroll
+  for (int i = 0; i < 4; i++)
+    asm volatile("st.global.v2.b64 [%0], {%1, %2};" :: "l"(reinterpret_cast<char*>(dst) + 16 * i), "l"(w[2 * i]), "l"(w[2 * i + 1]) : "memory");
+}
 
+// Pass 0 counts every owner's packets and padded key bytes into owner_cursor.  Pass 1 reserves the same amounts again, from a
+// zeroed cursor, inside every owner's destination and writes there: the packets, and each key as whole 8 B words (every key range
+// is padded to 8 B and starts 8 B aligned; an arena entry is reserved in whole 8 B words, so reading kpad bytes stays inside it).
 __global__ void __launch_bounds__(256) k_pack_partials(const __grid_constant__ PackParams P) {
   const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
   const PackCell c = pack_cell(P, g);
   const uint32_t n = __popc(c.amask);
   const unsigned long long r = block_reserve(n != 0u, c.owner, n, n * c.kpad, P.owner_cursor, P.world);
   if (P.pass == 0 || !n) return;
-  uint64_t row = (P.owner_base[c.owner] >> 32) + (r >> 32);
-  uint32_t boff = (uint32_t)(r & 0xFFFFFFFFull);                          // inside this owner's key segment
-  for (uint32_t m = c.amask; m; m &= m - 1u, row++, boff += c.kpad) {
-    const PackPane pp = pack_pane(P, __ffs(m) - 1);
-    P.entries[row] = pack_entry(pp, g, boff, c);
+  const PackDest d = P.dest[c.owner];
+  if (!d.entries) return;                                                 // the owner's ring overflowed: nothing is written
+  PartialEntry* out = d.entries + (r >> 32);
+  uint32_t key_off = d.key_off0 + (uint32_t)(r & 0xFFFFFFFFull);
+  for (uint32_t m = c.amask; m; m &= m - 1u, out++, key_off += c.kpad) {
+    store_packet(out, pack_entry(P, __ffs(m) - 1, g, key_off, c));
     if (!c.null_key) {
-      uint8_t* dst = P.key_bytes + (P.owner_base[c.owner] & 0xFFFFFFFFull) + boff;
+      uint64_t* dst = reinterpret_cast<uint64_t*>(d.keys + key_off);
       if (c.klen <= (uint32_t)INLINE_KEY) {
-        const uint64_t w[2] = {c.gk.k0, c.gk.k1};
-        for (uint32_t i = 0; i < c.klen; i++) dst[i] = (uint8_t)(w[i >> 3] >> ((i & 7) * 8));
+        for (uint32_t i = 0; i < c.kpad / 8u; i++) dst[i] = i ? c.gk.k1 : c.gk.k0;
       } else {
-        const uint8_t* src = P.dict.arena + c.gk.k1;
-        for (uint32_t i = 0; i < c.klen; i++) dst[i] = src[i];
+        const uint64_t* src = reinterpret_cast<const uint64_t*>(P.dict.arena + c.gk.k1);
+        for (uint32_t i = 0; i < c.kpad / 8u; i++) dst[i] = src[i];
       }
     }
   }
@@ -136,72 +138,30 @@ cudaError_t launch_merge_partials(const MergeParams& p, cudaStream_t s) {
 //   [wait: owners have merged step-2]      interprocess CUDA events, no spinning kernel
 //   k_pack_partials (pass 0)   per-owner packet / key-byte counts of the panes that closed under the global watermark
 //   k_xchg_reserve             one thread per owner: reserve the counted range in the OWNER'S ring with one remote atomicAdd
-//   k_pack_write_peer          write the packets and their key bytes straight into the owners' rings with P2P stores
+//   k_pack_partials (pass 1)   write the packets and their key bytes straight into the owners' rings with P2P stores
 //   [record: my packets of this step are written]  /  [wait: every peer's packets are written]
 //   k_merge_ring               intern unknown keys, merge the received partial states into the owner's panes
 //   [reset the ring half; record: merged]
 //   k_emit ...                 the owner emits the closed windows of ITS keys
 // =================================================================================================
-__global__ void k_xchg_reserve(XchgView X, unsigned long long* owner_cursor, unsigned long long* owner_base, unsigned long long* sent_total, uint32_t* err) {
+__global__ void k_xchg_reserve(XchgView X, unsigned long long* owner_cursor, PackDest* dest, unsigned long long* sent_total, uint32_t* err) {
   const int o = threadIdx.x;
   if (o >= X.world || o == X.rank) return;
   const unsigned long long c = owner_cursor[o];
-  unsigned long long base = 0;
-  if (c) {
-    base = atomicAdd_system(&X.peer[o].ctl->cursor[X.step & 1], c);
-    if ((base >> 32) + (c >> 32) > X.ring_entries || (base & 0xFFFFFFFFull) + (c & 0xFFFFFFFFull) > X.ring_key_bytes) {
-      atomicOr(&X.self.ctl->error, 1u); atomicOr(err, 0x100u);   // the owner's ring is too small for this step: nothing of it is written
-      base = ~0ull;
-    }
-  }
-  owner_base[o] = base;
   owner_cursor[o] = 0ull;
   atomicAdd(sent_total, c >> 32);
-}
-cudaError_t launch_xchg_reserve(const XchgView& X, unsigned long long* owner_cursor, unsigned long long* owner_base, unsigned long long* sent_total, uint32_t* err, cudaStream_t s) {
-  k_xchg_reserve<<<1, MAX_WORLD, 0, s>>>(X, owner_cursor, owner_base, sent_total, err);
-  return cudaGetLastError();
-}
-
-// pass 1 of the fused path: like k_pack_partials' write pass, but the destination is the owner's ring and key_off is absolute
-// A 64 B packet leaves as four 128-bit stores, the widest store sm_90 has (a peer write travels NVLink per store instruction).
-__device__ __forceinline__ void store_packet(PartialEntry* dst, const PartialEntry& e) {
-  const unsigned long long* w = reinterpret_cast<const unsigned long long*>(&e);
-#pragma unroll
-  for (int i = 0; i < 4; i++)
-    asm volatile("st.global.v2.b64 [%0], {%1, %2};" :: "l"(reinterpret_cast<char*>(dst) + 16 * i), "l"(w[2 * i]), "l"(w[2 * i + 1]) : "memory");
-}
-__global__ void __launch_bounds__(256) k_pack_write_peer(const __grid_constant__ PackParams P, const __grid_constant__ XchgView X, const unsigned long long* __restrict__ owner_base) {
-  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-  PackCell c = pack_cell(P, g);
-  unsigned long long base = 0ull;
-  if (c.amask) { base = owner_base[c.owner]; if (base == ~0ull) c.amask = 0u; }      // the owner's ring overflowed: nothing is written
-  const uint32_t n = __popc(c.amask);
-  const unsigned long long r = block_reserve(n != 0u, c.owner, n, n * c.kpad, P.owner_cursor, P.world);
-  if (!n) return;
-  const int half = (int)(X.step & 1);
-  uint64_t row = (base >> 32) + (r >> 32);
-  uint64_t boff = (base & 0xFFFFFFFFull) + (r & 0xFFFFFFFFull);           // inside the owner's key half
-  PartialEntry* ring = X.peer[c.owner].entries + (uint64_t)half * X.ring_entries;
-  uint8_t* keys = X.peer[c.owner].keys + (uint64_t)half * X.ring_key_bytes;
-  for (uint32_t m = c.amask; m; m &= m - 1u, row++, boff += c.kpad) {
-    const PackPane pp = pack_pane(P, __ffs(m) - 1);
-    store_packet(ring + row, pack_entry(pp, g, (uint32_t)boff, c));
-    if (!c.null_key) {
-      uint8_t* dst = keys + boff;
-      if (c.klen <= (uint32_t)INLINE_KEY) {
-        const uint64_t w[2] = {c.gk.k0, c.gk.k1};
-        for (uint32_t i = 0; i < c.kpad; i += 8) *reinterpret_cast<uint64_t*>(dst + i) = w[i >> 3];   // 8 B aligned: key ranges are padded to 8
-      } else {
-        const uint8_t* src = P.dict.arena + c.gk.k1;                                                  // arena entries are 8 B aligned and padded
-        for (uint32_t i = 0; i < c.kpad; i += 8) *reinterpret_cast<uint64_t*>(dst + i) = *reinterpret_cast<const uint64_t*>(src + i);
-      }
-    }
+  dest[o].entries = nullptr;
+  if (!c) return;
+  const unsigned long long base = atomicAdd_system(&X.peer[o].ctl->cursor[X.step & 1], c);
+  const uint64_t half = X.step & 1, row0 = base >> 32, byte0 = base & 0xFFFFFFFFull;
+  if (row0 + (c >> 32) > X.ring_entries || byte0 + (c & 0xFFFFFFFFull) > X.ring_key_bytes) {
+    atomicOr(&X.self.ctl->error, 1u); atomicOr(err, 0x100u);   // the owner's ring is too small for this step: nothing of it is written
+    return;
   }
+  dest[o] = PackDest{X.peer[o].entries + half * X.ring_entries + row0, X.peer[o].keys + half * X.ring_key_bytes, (uint32_t)byte0, 0u};
 }
-cudaError_t launch_pack_write_peer(const PackParams& p, const XchgView& X, const unsigned long long* owner_base, cudaStream_t s) {
-  if (!p.n_groups) return cudaSuccess;
-  k_pack_write_peer<<<(p.n_groups + 255) / 256, 256, 0, s>>>(p, X, owner_base);
+cudaError_t launch_xchg_reserve(const XchgView& X, unsigned long long* owner_cursor, PackDest* dest, unsigned long long* sent_total, uint32_t* err, cudaStream_t s) {
+  k_xchg_reserve<<<1, MAX_WORLD, 0, s>>>(X, owner_cursor, dest, sent_total, err);
   return cudaGetLastError();
 }
 

@@ -9,6 +9,20 @@
 
 // ------------------------------------------------------------------------------------------------
 // pane exchange (see include/dnz_gpu.h)
+namespace {
+// One pack launch per PACK_PANES panes of `send` (one thread per group id walks the panes of its launch).
+template <class Launch> void for_pane_chunks(PackParams& P, const std::vector<Pane*>& send, Launch&& launch) {
+  for (size_t i0 = 0; i0 < send.size(); i0 += PACK_PANES) {
+    P.n_panes = (int32_t)std::min<size_t>(PACK_PANES, send.size() - i0);
+    for (int j = 0; j < P.n_panes; j++) {
+      const Pane* p = send[i0 + j];
+      P.st[j] = p->st.as<GroupState>(); P.nullrows[j] = p->nullrows.as<unsigned long long>(); P.fz[j] = p->fz.as<unsigned long long>(); P.pane[j] = p->id;
+    }
+    launch();
+  }
+}
+}  // namespace
+
 void dnz_window::export_partials(int64_t watermark, dnz_partials* out) {
   process_pending(); drain();
   memset(out, 0, sizeof *out);
@@ -26,18 +40,15 @@ void dnz_window::export_partials(int64_t watermark, dnz_partials* out) {
   if (send.empty()) return;
   fetch_ctl();
   if (n_groups_host == 0) return;
-  d_owner_cursor.reserve((size_t)world * 8);
-  h_small.reserve((size_t)std::max(256, world * 8));
+  d_owner_cursor.reserve((size_t)world * 8); d_pack_dest.reserve((size_t)world * sizeof(PackDest));
+  h_small.reserve((size_t)std::max<size_t>(256, world * sizeof(PackDest)));
   PackParams P; memset(&P, 0, sizeof P);
   P.n_groups = n_groups_host; P.rank = rank; P.world = world; P.dict = dict_view();
-  P.owner_cursor = d_owner_cursor.as<unsigned long long>();
+  P.owner_cursor = d_owner_cursor.as<unsigned long long>(); P.dest = d_pack_dest.as<PackDest>();
   auto run_pass = [&](int pass) {
     CK(cudaMemsetAsync(d_owner_cursor.p, 0, (size_t)world * 8, stream));
     P.pass = pass;
-    for (Pane* p : send) {
-      P.st = p->st.as<GroupState>(); P.nullrows = p->nullrows.as<unsigned long long>(); P.fz = p->fz.as<unsigned long long>(); P.pane = p->id;
-      CK(launch_pack_partials(P, stream)); stats.total_launches++;
-    }
+    for_pane_chunks(P, send, [&] { CK(launch_pack_partials(P, stream)); stats.total_launches++; });
   };
   run_pass(0);
   CK(cudaMemcpyAsync(h_small.p, d_owner_cursor.p, (size_t)world * 8, cudaMemcpyDeviceToHost, stream));
@@ -46,13 +57,18 @@ void dnz_window::export_partials(int64_t watermark, dnz_partials* out) {
   for (int o = 0; o < world; o++) {
     uint64_t c = h_small.as<uint64_t>()[o];
     h_owner_counts[(size_t)o] = (int64_t)(c >> 32); h_owner_bytes[(size_t)o] = (int64_t)(c & 0xFFFFFFFFull);
-    P.owner_base[o] = (n_total << 32) | b_total;
     n_total += c >> 32; b_total += c & 0xFFFFFFFFull;
     if (n_total >= (1ull << 31) || b_total >= (1ull << 31)) fail(DNZ_ERR_UNSUPPORTED, "more than 2^31 packets or key bytes in one exchange step");
   }
   if (n_total == 0) return;
   d_part_entries.reserve((size_t)n_total * sizeof(PartialEntry)); d_part_keys.reserve((size_t)b_total + 64);
-  P.entries = d_part_entries.as<PartialEntry>(); P.key_bytes = d_part_keys.as<uint8_t>();
+  PackDest* dest = h_small.as<PackDest>();                     // the owners' segments, in rank order
+  int64_t n_seg = 0, b_seg = 0;
+  for (int o = 0; o < world; o++) {
+    dest[o] = PackDest{d_part_entries.as<PartialEntry>() + n_seg, d_part_keys.as<uint8_t>() + b_seg, 0u, 0u};
+    n_seg += h_owner_counts[(size_t)o]; b_seg += h_owner_bytes[(size_t)o];
+  }
+  CK(cudaMemcpyAsync(d_pack_dest.p, dest, (size_t)world * sizeof(PackDest), cudaMemcpyHostToDevice, stream));
   run_pass(1);
   CK(cudaStreamSynchronize(stream));
   out->n_entries = (int64_t)n_total; out->entries = d_part_entries.as<uint8_t>();
@@ -125,7 +141,7 @@ struct dnz_group {
   cudaEvent_t ev_packed[MAX_WORLD][2] = {}, ev_merged[MAX_WORLD][2] = {};
   XchgView view{};
   unsigned long long step = 0;
-  DevBuf d_owner_cursor, d_owner_base, d_totals;   // totals: [0] packets sent, [1] packets merged
+  DevBuf d_owner_cursor, d_pack_dest, d_totals;   // totals: [0] packets sent, [1] packets merged
   PinnedBuf h_totals; cudaEvent_t totals_ev = nullptr; bool totals_issued = false;
   int phase = 0;                                 // 0 idle, 1 begun, 2 packed
   // DNZ_TRACE: device timestamps of the step phases (pack start, packed, peers' packets seen, merged, emitted)
@@ -175,7 +191,7 @@ void group_alloc_region(dnz_group* g, unsigned event_flags) {
   CK(cudaSetDevice(g->dev));
   CK(cudaMalloc(&g->region, g->region_bytes));
   CK(cudaMemset(g->region, 0, 4096));
-  g->d_owner_cursor.alloc(MAX_WORLD * 8); g->d_owner_base.alloc(MAX_WORLD * 8); g->d_totals.alloc(64);
+  g->d_owner_cursor.alloc(MAX_WORLD * 8); g->d_pack_dest.alloc(MAX_WORLD * sizeof(PackDest)); g->d_totals.alloc(64);
   CK(cudaMemset(g->d_totals.p, 0, 64));
   g->h_totals.reserve(64); memset(g->h_totals.p, 0, 64);
   CK(cudaEventCreateWithFlags(&g->totals_ev, cudaEventDisableTiming));
@@ -286,22 +302,14 @@ void dnz_window::group_pack(dnz_group* g) {
   CK(cudaMemsetAsync(g->d_owner_cursor.p, 0, MAX_WORLD * 8, stream));
   PackParams P; memset(&P, 0, sizeof P);
   P.n_groups = gcap; P.rank = rank; P.world = world; P.dict = dict_view();      // grid bound; the kernels clamp to the device counter
-  P.owner_cursor = g->d_owner_cursor.as<unsigned long long>();
-  auto for_pane_chunks = [&](auto&& launch) {                 // up to PACK_PANES panes per launch (one thread per group id walks them)
-    for (size_t i0 = 0; i0 < send.size(); i0 += PACK_PANES) {
-      P.n_multi = (int32_t)std::min<size_t>(PACK_PANES, send.size() - i0);
-      for (int j = 0; j < P.n_multi; j++) {
-        Pane* p = send[i0 + j];
-        P.mst[j] = p->st.as<GroupState>(); P.mnull[j] = p->nullrows.as<unsigned long long>(); P.mfz[j] = p->fz.as<unsigned long long>(); P.mpane[j] = p->id;
-      }
-      launch(); stats.total_launches++;
-    }
-  };
+  P.owner_cursor = g->d_owner_cursor.as<unsigned long long>(); P.dest = g->d_pack_dest.as<PackDest>();
+  auto pack = [&] { CK(launch_pack_partials(P, stream)); stats.total_launches++; };
   P.pass = 0;
-  for_pane_chunks([&]() { CK(launch_pack_partials(P, stream)); });
-  CK(launch_xchg_reserve(X, g->d_owner_cursor.as<unsigned long long>(), g->d_owner_base.as<unsigned long long>(), g->d_totals.as<unsigned long long>(), &ctl()->merge_err, stream));
+  for_pane_chunks(P, send, pack);
+  CK(launch_xchg_reserve(X, g->d_owner_cursor.as<unsigned long long>(), g->d_pack_dest.as<PackDest>(), g->d_totals.as<unsigned long long>(), &ctl()->merge_err, stream));
   stats.total_launches++;
-  for_pane_chunks([&]() { CK(launch_pack_write_peer(P, X, g->d_owner_base.as<unsigned long long>(), stream)); });
+  P.pass = 1;
+  for_pane_chunks(P, send, pack);
   CK(cudaEventRecord(g->ev_packed[rank][par], stream));                    // "all my packets of this step are in the owners' rings"
   g->tmark(1, stream);
   g->hctl->packed[(int)(step & 3)][g->rank].store((int64_t)step, std::memory_order_release);

@@ -19,6 +19,8 @@ namespace dnz {
 
 // SMs of an H100 SXM: the grid-stride utility kernels that are not handed the device's SM count launch a multiple of it
 constexpr int GRID_SMS = 132;
+// blocks of 256 threads for a grid-stride kernel over n items: one item per thread, at most `per_sm` blocks per SM
+static unsigned stride_grid(uint64_t n, int per_sm) { return (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)GRID_SMS * per_sm); }
 
 // =================================================================================================
 // k_tile_scan
@@ -608,17 +610,13 @@ __global__ void __launch_bounds__(256) k_merge_private(const __grid_constant__ A
   if (g >= P.priv_groups) return;
   GroupState* dst = P.panes.main[pi];
   if (!dst) return;
-  double cnt = 0.0, sum = 0.0; unsigned long long mn = 0, mx = 0; bool first = true;
-  for (int c = 0; c < n_cta; c++) {
-    const GroupState s = P.priv[((size_t)c * P.panes.n_panes + pi) * P.priv_groups + g];
-    if (s.cnt != 0.0) { sum = first ? s.sum : sum + s.sum; first = false; cnt += s.cnt; }
-    mn = max(mn, s.minkey); mx = max(mx, s.maxkey);
-  }
-  if (cnt == 0.0) return;
+  StateFold<double> f;
+  for (int c = 0; c < n_cta; c++) f.add(P.priv[((size_t)c * P.panes.n_panes + pi) * P.priv_groups + g]);
+  if (f.cnt == 0.0) return;
   GroupState* d = dst + g;                      // the slow paths may have reduced into the pane concurrently-ordered before: add
-  red_add_f64(&d->cnt, cnt); red_add_f64(&d->sum, sum);
-  if (mn) red_max_u64(&d->minkey, mn);
-  if (mx) red_max_u64(&d->maxkey, mx);
+  red_add_f64(&d->cnt, f.cnt); red_add_f64(&d->sum, f.sum);
+  if (f.mnk) red_max_u64(&d->minkey, f.mnk);
+  if (f.mxk) red_max_u64(&d->maxkey, f.mxk);
 }
 cudaError_t launch_merge_private(const AggParams& p, int grid, cudaStream_t s) {
   if (!p.priv || grid <= 0) return cudaSuccess;
@@ -635,8 +633,7 @@ cudaError_t launch_aggregate_generic(const AggParams& p, int sm_count, cudaStrea
 }
 cudaError_t launch_deferred(const AggParams& p, const DeferEntry* in, uint64_t n_entries, cudaStream_t s) {
   if (!n_entries) return cudaSuccess;
-  uint64_t gb = (n_entries + 255) / 256; int grid = (int)(gb < GRID_SMS * 8 ? gb : GRID_SMS * 8);
-  k_deferred<<<grid, 256, 0, s>>>(p, n_entries, in);
+  k_deferred<<<stride_grid(n_entries, 8), 256, 0, s>>>(p, n_entries, in);
   return cudaGetLastError();
 }
 
@@ -655,7 +652,8 @@ __device__ __forceinline__ void uacc_add(UAcc& a, bool val_ok, double v) {
   const unsigned long long o = ord_bits((unsigned long long)__double_as_longlong(v));
   a.cnt += 1.0; a.sum += v; a.mink = max(a.mink, ~o); a.maxk = max(a.maxk, o);
 }
-__device__ void uacc_flush(UAcc& a, GroupState* m, GroupState* l, unsigned long long* nm, unsigned long long* nl, double* s_red) {
+__device__ void uacc_flush(UAcc& a, GroupState* m, GroupState* l, unsigned long long* nm, unsigned long long* nl,
+                           GroupState* s_part, unsigned long long* s_nulls) {
   // block reduction (256 threads): warp shuffles, then warp 0 over the 8 partials
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int o = 16; o; o >>= 1) {
@@ -663,27 +661,25 @@ __device__ void uacc_flush(UAcc& a, GroupState* m, GroupState* l, unsigned long 
     a.mink = max(a.mink, __shfl_xor_sync(0xffffffffu, a.mink, o)); a.maxk = max(a.maxk, __shfl_xor_sync(0xffffffffu, a.maxk, o));
     a.nulls += __shfl_xor_sync(0xffffffffu, a.nulls, o);
   }
-  unsigned long long* s_u = reinterpret_cast<unsigned long long*>(s_red);
   __syncthreads();
-  if (lane == 0) { s_red[warp * 5 + 0] = a.cnt; s_red[warp * 5 + 1] = a.sum; s_u[warp * 5 + 2] = a.mink; s_u[warp * 5 + 3] = a.maxk; s_u[warp * 5 + 4] = a.nulls; }
+  if (lane == 0) { s_part[warp] = GroupState{a.cnt, a.sum, a.mink, a.maxk}; s_nulls[warp] = a.nulls; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    double cnt = 0, sum = 0; unsigned long long mink = 0, maxk = 0, nulls = 0; bool first = true;
-    for (int w = 0; w < 8; w++) {
-      if (s_red[w * 5] != 0.0) { sum = first ? s_red[w * 5 + 1] : sum + s_red[w * 5 + 1]; first = false; cnt += s_red[w * 5]; }
-      mink = max(mink, s_u[w * 5 + 2]); maxk = max(maxk, s_u[w * 5 + 3]); nulls += s_u[w * 5 + 4];
-    }
+    StateFold<double> f; unsigned long long nulls = 0;
+#pragma unroll 1                                  // once per pane change: unrolled, the eight loads would cost the kernel registers
+    for (int w = 0; w < 8; w++) { f.add(s_part[w]); nulls += s_nulls[w]; }
     for (int k = 0; k < 2; k++) {
       GroupState* d = k ? l : m; unsigned long long* dn = k ? nl : nm;
       if (!d) continue;
-      if (cnt != 0.0) { red_add_f64(&d->cnt, cnt); red_add_f64(&d->sum, sum); red_max_u64(&d->minkey, mink); red_max_u64(&d->maxkey, maxk); }
+      if (f.cnt != 0.0) { red_add_f64(&d->cnt, f.cnt); red_add_f64(&d->sum, f.sum); red_max_u64(&d->minkey, f.mnk); red_max_u64(&d->maxkey, f.mxk); }
       if (nulls && dn) red_add_u64(dn, nulls);
     }
   }
   a.cnt = 0; a.sum = 0; a.mink = 0; a.maxk = 0; a.nulls = 0;
 }
 __global__ void __launch_bounds__(256) k_aggregate_ungrouped(const __grid_constant__ AggParams P) {
-  __shared__ double s_red[8 * 5];
+  __shared__ GroupState s_part[8];
+  __shared__ unsigned long long s_nulls[8];
   const int64_t n_tiles = P.tile_end - P.tile_begin;
   const int64_t chunk = (n_tiles + gridDim.x - 1) / gridDim.x;
   const int64_t t0 = P.tile_begin + (int64_t)blockIdx.x * chunk, t1 = min(P.tile_end, t0 + chunk);
@@ -692,7 +688,7 @@ __global__ void __launch_bounds__(256) k_aggregate_ungrouped(const __grid_consta
   auto flush = [&]() {
     if (cur == INT64_MIN) return;
     const int64_t pi = cur - P.panes.pane0;
-    if (pi >= 0 && pi < P.panes.n_panes) uacc_flush(a, P.panes.main[pi], P.panes.late[pi], P.panes.nullrows_main[pi], P.panes.nullrows_late[pi], s_red);
+    if (pi >= 0 && pi < P.panes.n_panes) uacc_flush(a, P.panes.main[pi], P.panes.late[pi], P.panes.nullrows_main[pi], P.panes.nullrows_late[pi], s_part, s_nulls);
     cur = INT64_MIN;
   };
   for (int64_t t = t0; t < t1; t++) {
@@ -727,16 +723,13 @@ __global__ void k_ungrouped_collect(const UWindow* __restrict__ wins, int n, USt
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const UWindow w = wins[i];
-  UState r; r.cnt = 0; r.sum = 0.0; r.mink = 0; r.maxk = 0; r.nulls = 0;
-  bool first = true;
+  StateFold<unsigned long long> f; unsigned long long nulls = 0;
   for (int p = 0; p < w.n; p++) {
     if (!w.st[p]) continue;
-    const GroupState s = *w.st[p];
-    if (s.cnt != 0.0) { r.sum = first ? s.sum : r.sum + s.sum; first = false; r.cnt += (unsigned long long)s.cnt; }
-    r.mink = max(r.mink, s.minkey); r.maxk = max(r.maxk, s.maxkey);
-    if (w.nr[p]) r.nulls += *w.nr[p];
+    f.add(*w.st[p]);
+    if (w.nr[p]) nulls += *w.nr[p];
   }
-  out[i] = r;
+  out[i] = UState{f.cnt, f.sum, f.mnk, f.mxk, nulls};
 }
 cudaError_t launch_ungrouped_collect(const UWindow* wins, int n, UState* out, cudaStream_t s) {
   if (n <= 0) return cudaSuccess;
@@ -760,24 +753,17 @@ __device__ __forceinline__ bool predicate(int op, long long a, long long b) {
   switch (op) { case 0: return a > b; case 1: return a >= b; case 2: return a < b; case 3: return a <= b; case 4: return a == b; default: return a != b; }
 }
 
-// owner hash of a group's key (NULL key: 0 -> rank 0)
-__device__ __forceinline__ uint64_t key_hash(const GidKey& gk) {
-  if (gk.len == 0xFFFFFFFFu) return 0;
-  return gk.len <= (uint32_t)INLINE_KEY ? hash_inline(gk.k0, gk.k1, gk.len) : gk.k0;
-}
-
 struct Combined { unsigned long long cnt, nullrows, mnk, mxk, fz; double sum; bool present; };   // cnt: exact integer
 
 __device__ __forceinline__ Combined combine_panes(const EmitParams& P, uint32_t g) {
-  Combined c; c.cnt = 0; c.nullrows = 0; c.mnk = 0; c.mxk = 0; c.fz = ~0ull; c.sum = 0.0;
-  bool first = true;
+  StateFold<unsigned long long> f;
+  Combined c; c.nullrows = 0; c.fz = ~0ull;
   for (int p = 0; p < P.n_panes; p++) {
-    const GroupState s = P.panes[p][g];
-    if (s.cnt != 0.0) { c.sum = first ? s.sum : c.sum + s.sum; first = false; }   // no "+ 0.0" for absent panes: keeps -0.0 sums exact
-    c.cnt += (unsigned long long)s.cnt; c.mnk = max(c.mnk, s.minkey); c.mxk = max(c.mxk, s.maxkey);
+    f.add(P.panes[p][g]);
     if (P.nullrows[p]) c.nullrows += P.nullrows[p][g];
     if (P.fz[p]) c.fz = min(c.fz, P.fz[p][g]);
   }
+  c.cnt = f.cnt; c.sum = f.sum; c.mnk = f.mnk; c.mxk = f.mxk;
   c.present = (c.cnt | c.nullrows) != 0;
   return c;
 }
@@ -802,7 +788,7 @@ __global__ void __launch_bounds__(256) k_emit(const __grid_constant__ EmitParams
     if (c.present) {
       gk = P.dict.gid_key[g];
       klen = gk.len == 0xFFFFFFFFu ? 0u : gk.len;
-      keep = P.world <= 1 || (int)(key_hash(gk) % (uint64_t)P.world) == P.rank;
+      keep = P.world <= 1 || key_owner(gk, P.world) == P.rank;
       agg_ok = c.cnt != 0;
       if (agg_ok) {
         unsigned long long bmn = unord_bits(ORD_F64_MAX - c.mnk), bmx = unord_bits(c.mxk + ORD_F64_MIN);
@@ -998,16 +984,6 @@ bool ts_format_supported(const char* fmt) {
 // =================================================================================================
 // small utilities
 // =================================================================================================
-__global__ void k_fill_u64(unsigned long long* p, uint64_t n, unsigned long long v) {
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) p[i] = v;
-}
-cudaError_t launch_fill_u64(unsigned long long* p, uint64_t n, unsigned long long v, cudaStream_t s) {
-  if (!n) return cudaSuccess;
-  uint64_t gb = (n + 255) / 256; int grid = (int)(gb < GRID_SMS * 16 ? gb : GRID_SMS * 16);
-  k_fill_u64<<<grid, 256, 0, s>>>(p, n, v);
-  return cudaGetLastError();
-}
-
 // Host-pinned -> device gather copy.  CTAs claim 256 KiB pieces of the descriptor list dynamically; every thread keeps
 // eight 16 B loads from system memory in flight (PCIe reads need ~100 KB outstanding to reach line rate).
 __global__ void __launch_bounds__(256) k_gather_copy(const CopyDesc* __restrict__ descs, uint32_t n, unsigned int* cursor) {
@@ -1056,48 +1032,27 @@ cudaError_t launch_gather_copy(const CopyDesc* descs, uint32_t n, unsigned int* 
 // re-insert every occupied slot of the old table into the (zeroed) new one; group ids are preserved
 __global__ void k_dict_rehash(const DictSlot* old_slots, uint32_t old_cap, DictView nd) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < old_cap; i += (uint64_t)gridDim.x * blockDim.x) {
-    DictSlot s = old_slots[i];
+    const DictSlot s = old_slots[i];
     if (s.state == SLOT_EMPTY || s.state == SLOT_LOCKED) continue;
-    uint64_t h = s.len <= (uint32_t)INLINE_KEY ? hash_inline(s.k0, s.k1, s.len) : s.k0;
-    uint32_t idx = (uint32_t)h & nd.mask;
-    for (;;) {
-      uint32_t old = atomicCAS(&nd.slots[idx].state, SLOT_EMPTY, SLOT_LOCKED);
-      if (old == SLOT_EMPTY) break;
-      idx = (idx + 1) & nd.mask;
-    }
-    DictSlot* d = nd.slots + idx;
-    d->k0 = s.k0; d->k1 = s.k1; d->hint = s.hint; d->len = s.len;
-    __threadfence();
-    d->state = s.state;
+    dict_place(nd, stored_key_hash(s.k0, s.k1, s.len), s.k0, s.k1, s.len, s.hint, s.state);
   }
 }
 cudaError_t launch_dict_rehash(const DictSlot* old_slots, uint32_t old_cap, DictView nd, cudaStream_t s) {
-  uint64_t gb = ((uint64_t)old_cap + 255) / 256; int grid = (int)(gb < GRID_SMS * 16 ? gb : GRID_SMS * 16);
-  k_dict_rehash<<<grid, 256, 0, s>>>(old_slots, old_cap, nd);
+  k_dict_rehash<<<stride_grid(old_cap, 16), 256, 0, s>>>(old_slots, old_cap, nd);
   return cudaGetLastError();
 }
-
 
 // checkpoint restore: re-insert the keys of gid_key[0, n) into an EMPTY table with their original group ids
 __global__ void k_dict_restore(DictView d, uint32_t n) {
   for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < n; g += gridDim.x * blockDim.x) {
     const GidKey gk = d.gid_key[g];
     if (gk.len == 0xFFFFFFFFu) { *d.null_gid = g + 1; continue; }
-    const uint64_t h = gk.len <= (uint32_t)INLINE_KEY ? hash_inline(gk.k0, gk.k1, gk.len) : gk.k0;
-    uint32_t idx = (uint32_t)h & d.mask;
-    for (;;) {
-      if (atomicCAS(&d.slots[idx].state, SLOT_EMPTY, SLOT_LOCKED) == SLOT_EMPTY) break;
-      idx = (idx + 1) & d.mask;
-    }
-    DictSlot* s = d.slots + idx;
-    s->k0 = gk.k0; s->k1 = gk.k1; s->hint = 0; s->len = gk.len;
-    __threadfence();
-    s->state = g + 1;
+    dict_place(d, stored_key_hash(gk.k0, gk.k1, gk.len), gk.k0, gk.k1, gk.len, 0ull, g + 1);
   }
 }
 cudaError_t launch_dict_restore(DictView d, uint32_t n, cudaStream_t s) {
   if (!n) return cudaSuccess;
-  k_dict_restore<<<(unsigned)std::min<uint64_t>(((uint64_t)n + 255) / 256, GRID_SMS * 16), 256, 0, s>>>(d, n);
+  k_dict_restore<<<stride_grid(n, 16), 256, 0, s>>>(d, n);
   return cudaGetLastError();
 }
 
@@ -1105,8 +1060,7 @@ __global__ void k_clear_hints(DictSlot* slots, uint32_t cap) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < cap; i += (uint64_t)gridDim.x * blockDim.x) slots[i].hint = 0;
 }
 cudaError_t launch_clear_hints(DictSlot* slots, uint32_t cap, cudaStream_t s) {
-  uint64_t gb = ((uint64_t)cap + 255) / 256; int grid = (int)(gb < GRID_SMS * 16 ? gb : GRID_SMS * 16);
-  k_clear_hints<<<grid, 256, 0, s>>>(slots, cap);
+  k_clear_hints<<<stride_grid(cap, 16), 256, 0, s>>>(slots, cap);
   return cudaGetLastError();
 }
 

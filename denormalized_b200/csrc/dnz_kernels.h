@@ -111,6 +111,19 @@ struct __align__(32) GroupState {
   unsigned long long maxkey;   // ord(v) - ORD(f64::MIN): 0 == f64::MIN
 };
 
+// ord(): monotone map f64 -> u64 over IEEE totalOrder.  min/max accumulators are kept as distances from the
+// DataFusion starting values (f64::MAX for min, f64::MIN for max) so that a zero-filled state IS the start.
+constexpr unsigned long long SIGN64 = 0x8000000000000000ull;
+constexpr unsigned long long BITS_F64_MAX = 0x7FEFFFFFFFFFFFFFull;
+constexpr unsigned long long ORD_F64_MAX = BITS_F64_MAX | SIGN64;        // ord(+MAX)
+constexpr unsigned long long ORD_F64_MIN = ~(BITS_F64_MAX | SIGN64);     // ord(-MAX)
+__host__ __device__ __forceinline__ unsigned long long ord_bits(unsigned long long b) { return (b & SIGN64) ? ~b : (b | SIGN64); }
+__host__ __device__ __forceinline__ unsigned long long unord_bits(unsigned long long o) { return (o & SIGN64) ? (o & ~SIGN64) : ~o; }
+// IEEE totalOrder key (arrow-ord cmp on floats == f64::total_cmp)
+__host__ __device__ __forceinline__ long long total_key(unsigned long long b) {
+  long long s = (long long)b; return s ^ (long long)(((unsigned long long)(s >> 63)) >> 1);
+}
+
 struct PaneTable {             // uploaded per launch
   int64_t pane0;               // pane id of entry 0
   int32_t n_panes; int32_t pad;
@@ -178,16 +191,18 @@ struct __align__(16) PartialEntry {
 static_assert(sizeof(PartialEntry) == 64, "packet size");
 constexpr int MAX_WORLD = 32;
 constexpr int PACK_PANES = 32;       // panes per pack launch (a 32-bit mask per group id)
+// Where the write pass puts one owner's packets and key bytes: its segment of the local export buffers, or its reserved range
+// of the owner's receive ring.  `entries` is the first packet of the range; its key bytes start at keys + key_off0, and a
+// packet's key_off counts from `keys` (the segment: key_off0 = 0; the ring half: the reserved base).  entries == nullptr:
+// write nothing for this owner.
+struct PackDest { PartialEntry* entries; uint8_t* keys; uint32_t key_off0, pad; };
 struct PackParams {
-  const GroupState* st; const unsigned long long* nullrows; const unsigned long long* fz;   // one pane (host-driven export) ...
-  int64_t pane; uint32_t n_groups; int32_t rank, world;
-  // ... or up to PACK_PANES panes in one launch (fused exchange; one thread per group id walks them)
-  int32_t n_multi, pad_multi;
-  const GroupState* mst[PACK_PANES]; const unsigned long long* mnull[PACK_PANES]; const unsigned long long* mfz[PACK_PANES]; int64_t mpane[PACK_PANES];
+  uint32_t n_groups; int32_t rank, world, n_panes;
+  const GroupState* st[PACK_PANES]; const unsigned long long* nullrows[PACK_PANES]; const unsigned long long* fz[PACK_PANES];
+  int64_t pane[PACK_PANES];                      // up to PACK_PANES panes in one launch: one thread per group id walks them
   DictView dict;
-  PartialEntry* entries; uint8_t* key_bytes;     // pass 1 output, grouped by owner
-  unsigned long long* owner_cursor;              // [world] (entries << 32) | key bytes, running over all panes of the export
-  unsigned long long owner_base[MAX_WORLD];      // pass 1: (first entry << 32) | first key byte of every owner's segment
+  unsigned long long* owner_cursor;              // [world] (entries << 32) | key bytes, running over all launches of a pass
+  const PackDest* dest;                          // [world] write pass: every owner's destination
   int32_t pass;                                  // 0: count, 1: write
 };
 struct MergeParams {
@@ -214,7 +229,6 @@ struct UState { unsigned long long cnt; double sum; unsigned long long mink, max
 cudaError_t launch_ungrouped_collect(const UWindow* wins, int n, UState* out, cudaStream_t s);
 cudaError_t launch_deferred(const AggParams& p, const DeferEntry* in, uint64_t n_entries, cudaStream_t s);
 cudaError_t launch_emit(const EmitParams& p, cudaStream_t s);
-cudaError_t launch_fill_u64(unsigned long long* p, uint64_t n, unsigned long long v, cudaStream_t s);
 cudaError_t launch_dict_rehash(const DictSlot* old_slots, uint32_t old_cap, DictView nd, cudaStream_t s);
 cudaError_t launch_clear_hints(DictSlot* slots, uint32_t cap, cudaStream_t s);
 cudaError_t launch_dict_restore(DictView d, uint32_t n, cudaStream_t s);
@@ -236,8 +250,7 @@ struct XchgView {
   unsigned long long step;                    // 1, 2, ... (same on every rank)
   int32_t rank, world;
 };
-cudaError_t launch_xchg_reserve(const XchgView& X, unsigned long long* owner_cursor, unsigned long long* owner_base, unsigned long long* sent_total, uint32_t* err, cudaStream_t s);
-cudaError_t launch_pack_write_peer(const PackParams& p, const XchgView& X, const unsigned long long* owner_base, cudaStream_t s);
+cudaError_t launch_xchg_reserve(const XchgView& X, unsigned long long* owner_cursor, PackDest* dest, unsigned long long* sent_total, uint32_t* err, cudaStream_t s);
 cudaError_t launch_merge_ring(const MergeParams& p, const XchgView& X, unsigned long long* merged_total, int sm_count, cudaStream_t s);
 
 // Arrow<->device buffer manager: one launch pulls every pinned host buffer of a superbatch over PCIe with 128-bit loads

@@ -10,12 +10,7 @@ void reference_windows(int64_t mn, int64_t mx, int64_t L, int64_t S, std::vector
   if (S > 0) { for (int64_t cur = snap(mn - L); cur <= mx; cur += S) { const int64_t end = cur + L; if (mn > end || mx < cur) continue; out.push_back(cur); } }
   else for (int64_t cur = snap(mn); cur <= mx; cur += L) out.push_back(cur);
 }
-inline unsigned long long unord_bits_h(unsigned long long o) { return (o & 0x8000000000000000ull) ? (o & ~0x8000000000000000ull) : ~o; }
-inline int total_cmp_d(double a, double b) {
-  long long x, y; memcpy(&x, &a, 8); memcpy(&y, &b, 8);
-  x ^= (long long)(((unsigned long long)(x >> 63)) >> 1); y ^= (long long)(((unsigned long long)(y >> 63)) >> 1);
-  return x < y ? -1 : x > y ? 1 : 0;
-}
+inline long long total_key_of(double d) { unsigned long long b; memcpy(&b, &d, 8); return total_key(b); }
 }  // namespace
 
 // The Partial stage's emission schedule for one run (or a flush): per batch, the frames it creates and the frames its watermark
@@ -91,7 +86,7 @@ void dnz_window::ungrouped_final(const std::vector<URow>& pb) {
     if (x.valid) {
       f.sum += x.sum;
       if (!f.has) { f.mn = x.mn; f.mx = x.mx; f.has = true; }
-      else { if (total_cmp_d(x.mn, f.mn) < 0) f.mn = x.mn; if (total_cmp_d(x.mx, f.mx) > 0) f.mx = x.mx; }
+      else { if (total_key_of(x.mn) < total_key_of(f.mn)) f.mn = x.mn; if (total_key_of(x.mx) > total_key_of(f.mx)) f.mx = x.mx; }
     }
   }
   if (!u_has_fwm || start > u_fwm) { u_fwm = start; u_has_fwm = true; }
@@ -117,7 +112,7 @@ void dnz_window::ungrouped_collect(bool wait) {
       for (int64_t ws : pb) {
         const UState& u = st[k++];
         URow x; x.ws = ws; x.we = ws + L; x.cnt = (int64_t)u.cnt; x.valid = u.cnt != 0; x.sum = u.sum; x.avg = 0;
-        unsigned long long bmn = unord_bits_h(~u.mink), bmx = unord_bits_h(u.maxk);
+        unsigned long long bmn = unord_bits(~u.mink), bmx = unord_bits(u.maxk);
         memcpy(&x.mn, &bmn, 8); memcpy(&x.mx, &bmx, 8);
         rows.push_back(x);
       }

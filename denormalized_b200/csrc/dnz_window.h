@@ -325,7 +325,7 @@ struct dnz_window {
   bool group_started = false;                     // this operator has taken part in a group step (its stream has begun in the group)
   bool has_lwm = false; int64_t lwm = 0;          // local watermark (exchange mode: emission follows the GLOBAL one)
   int64_t exported_pane_upto = INT64_MIN;
-  DevBuf d_part_entries, d_part_keys, d_owner_cursor, d_xptrs; PinnedBuf h_xptrs;
+  DevBuf d_part_entries, d_part_keys, d_owner_cursor, d_pack_dest, d_xptrs; PinnedBuf h_xptrs;
   std::vector<int64_t> h_owner_counts, h_owner_bytes;
   void group_begin(struct dnz_group* g);
   void group_pack(struct dnz_group* g);
