@@ -27,6 +27,8 @@ FLAG_NO_HINTS = 4
 FLAG_NO_QUEUE = 8
 FLAG_NO_PRIVATE = 16
 FLAG_SYNCHRONOUS = 32
+FLAG_SCALAR_PROBE = 64
+FLAG_STAGE_TS = 128
 INTERNAL_METADATA_COLUMN = "_streaming_internal_metadata"   # crates/common/src/lib.rs:5
 
 

@@ -63,6 +63,24 @@ __device__ __forceinline__ void ld_slot(const DictSlot* p, uint64_t& a, uint64_t
   ld_relaxed_b128(&p->hint, c, d);
   ld_relaxed_b128(&p->k0, a, b);
 }
+// ld_slot for a warp, by lane pairs: lanes 2j / 2j+1 load the two 16 B halves of ONE slot per instruction, first the slot of
+// the even lane's row (the even lane its key words, the odd lane its {hint, len | state}), then the slot of the odd lane's row
+// (the odd lane its key words, the even lane its {hint, len | state}).  Each lane then holds its own key words and the other
+// half of its partner's slot, and one xor-shuffle of 16 B swaps those.  A warp's 32 probes cost two instructions of 16 sector
+// requests each instead of two of 32.  The halves stay two unordered loads (by two lanes now), so the torn-read argument of
+// ld_slot holds unchanged.  Every lane of the warp calls it with a valid slot index `idx` (the loads are not predicated per
+// row: the caller skips the call when no row of the warp probes, and a row that does not probe ignores what it got).
+__device__ __forceinline__ void ld_slot_paired(const DictSlot* slots, uint32_t idx, uint32_t odd, uint64_t& a, uint64_t& b,
+                                               uint64_t& c, uint64_t& d) {
+  const uint32_t idx2 = __shfl_xor_sync(0xffffffffu, idx, 1);
+  const uint8_t* base = reinterpret_cast<const uint8_t*>(slots);
+  uint64_t x0, x1, y0, y1;
+  ld_relaxed_b128(base + (size_t)(odd ? idx2 : idx) * sizeof(DictSlot) + 16u * odd, x0, x1);
+  ld_relaxed_b128(base + (size_t)(odd ? idx : idx2) * sizeof(DictSlot) + 16u * (odd ^ 1u), y0, y1);
+  // x: the even lane's row, y: the odd lane's row
+  a = odd ? y0 : x0; b = odd ? y1 : x1;
+  c = __shfl_xor_sync(0xffffffffu, odd ? x0 : y0, 1); d = __shfl_xor_sync(0xffffffffu, odd ? x1 : y1, 1);
+}
 __device__ __forceinline__ void ld_slot_ordered(const DictSlot* p, uint64_t& a, uint64_t& b, uint64_t& c, uint64_t& d) {
   ld_acquire_b128(&p->hint, c, d);
   ld_relaxed_b128(&p->k0, a, b);

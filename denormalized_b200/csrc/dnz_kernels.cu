@@ -234,18 +234,19 @@ __global__ void __launch_bounds__(256) k_deferred(const __grid_constant__ AggPar
 //
 // The last warp is the TMA producer.  It claims tiles from a global counter (stream order), resolves their descriptors,
 // and per tile: waits for the ring slot, writes the tile header (row count, key byte base, resolved pane state array +
-// hint tag) into shared memory and issues four 1-D bulk copies (timestamps, values, key offsets, key bytes; SASS
-// UBLKCP) that complete on the slot's `full` mbarrier.
+// hint tag) into shared memory and issues 1-D bulk copies (values, key offsets, key bytes, and the timestamps only for
+// a tile that spans panes; SASS UBLKCP) that complete on the slot's `full` mbarrier.
 //
 // The other 13 warps consume, one row per thread (26 consumer warps per SM across the two CTAs hide the L2 round trip of
 // the probe).  Hot path per row: 3 LDS for value/offsets, 4-5 LDS.32 + funnel shifts + clamp-shift masks for the <= 16 B
-// key, a 32-bit hash, ONE probe of the 32 B dictionary slot (two independent 16 B loads of the same sector, LDG.E.128, see
-// ld_slot) that also carries the group's min/max hint; a row whose
+// key, a 32-bit hash, ONE probe of the 32 B dictionary slot by lane pairs (ld_slot_paired: two LDG.E.128 per warp, each
+// covering the whole slots of 16 rows, and one 16 B xor-shuffle) that also carries the group's min/max hint; a row whose
 // slot holds another key is parked in the warp's retry queue; count and sum are reduced by lane PAIRS: lanes 2j / 2j+1
 // update {cnt, sum} of the same row with one red.add.f64 (16 sectors per instruction instead of 32); min / max are reduced
 // by the row's own lane for the ~7 % of the rows the hint lets through.  Everything rare (empty or locked slot -> insert,
 // keys > 16 B, +-0.0 / non-finite values, tiles spanning panes, late panes) is outlined into __noinline__ helpers so
-// that the hot loop stays ~330 SASS instructions per 32 rows (profiles/README.md).
+// that the hot loop stays ~360 SASS instructions per 32 rows.  DNZ_FLAG_SCALAR_PROBE / DNZ_FLAG_STAGE_TS restore the per-row
+// probe and the timestamp copy of every tile for A/B runs.
 // =================================================================================================
 struct __align__(16) StageHdr {   // the consumers read the first two 16 B words with one LDS.128 each (2 wavefronts per tile, not 8)
   int32_t n_rows, flags, a0; uint32_t tag;
@@ -278,7 +279,7 @@ static_assert(TILE <= 1024, "row packing");
 struct __align__(16) TileFetch {     // what the producer needs to hand one tile to the ring (staged in shared memory, 2 x 32)
   StageHdr h;
   const int64_t* gts; const double* gval; const int32_t* goff; const uint8_t* gby;
-  uint32_t nts, noff, nby, pad;
+  uint32_t nval, nts, noff, nby;     // bytes of the four copies (nts = 0: the timestamps are not staged)
 };
 struct AggSmem {
   Stage st[STAGES];
@@ -305,9 +306,11 @@ __device__ __noinline__ uint64_t agg_probe_slow_global(const AggParams& P, const
   uint32_t slot = 0; uint32_t g = dict_lookup(P.dict, k, false, &slot);
   return ((uint64_t)slot << 32) | g;
 }
-// Accumulate one staged row through the general per-row path (pane from the timestamp, late panes, +-0.0, ...).
-__device__ __noinline__ void agg_apply_slow(const AggParams& P, const StageHdr& h, uint32_t r, long long ts, double v, uint32_t gid) {
-  long long pane = (h.flags & TILE_PANE_UNIFORM) ? h.pane_lo : ts / P.panes.pane_ms;
+// Accumulate one staged row through the general per-row path (pane from the timestamp, late panes, +-0.0, ...).  The
+// timestamps are staged only for tiles that span panes, so they are read only behind the TILE_PANE_UNIFORM test.
+__device__ __noinline__ void agg_apply_slow(const AggParams& P, const Stage& st, uint32_t r, double v, uint32_t gid) {
+  const StageHdr& h = st.hdr;
+  long long pane = (h.flags & TILE_PANE_UNIFORM) ? h.pane_lo : st.ts[r] / P.panes.pane_ms;
   apply_row(P, h.tile_rel, r, pane, true, v, gid, h.rowseq0 + r);
 }
 // Lookup / insert of a parked row whose chain ended in an empty or locked slot (inline key rebuilt from its words).
@@ -390,7 +393,7 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
     auto fetch = [&](int64_t t, TileFetch& d) {
       StageHdr h; h.mbase = nullptr; h.tag = 0; h.pane_lo = 0; h.rowseq0 = 0; h.n_rows = 0; h.flags = 0; h.a0 = 0; h.tile_rel = 0;
       h.pane_rel = 0; h.gbytes = nullptr; h.pad[0] = h.pad[1] = 0;
-      d.nts = d.noff = d.nby = 0;
+      d.nval = d.nts = d.noff = d.nby = 0;
       if (t < P.tile_end) {
         const TileDesc td = P.tiles[t];
         const BatchDesc& bd = P.batches[td.batch];
@@ -399,7 +402,9 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
         h.rowseq0 = ((unsigned long long)bd.seq << 32) | (unsigned long long)(uint32_t)td.row0;
         if (td.flags & TILE_FAST) {
           d.gts = bd.ts + td.row0; d.gval = bd.val + td.row0; d.goff = bd.off + td.row0; d.gby = bd.bytes + h.a0;
-          d.nts = round16((uint32_t)td.n_rows * 8u); d.noff = round16(((uint32_t)td.n_rows + 1u) * 4u);
+          // the consumers read a staged timestamp only to find the pane of a row of a tile that spans panes (agg_apply_slow)
+          d.nval = round16((uint32_t)td.n_rows * 8u); d.noff = round16(((uint32_t)td.n_rows + 1u) * 4u);
+          d.nts = ((td.flags & TILE_PANE_UNIFORM) && !(P.flags & AGG_STAGE_TS)) ? 0u : d.nval;
           d.nby = (td.flags & TILE_KEYS_GLOBAL) ? 0u : round16((uint32_t)(td.byte0 + td.byte_len - h.a0));
           h.gbytes = bd.bytes;
           if (td.flags & TILE_PANE_UNIFORM) {
@@ -438,9 +443,9 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
           mbar_wait(&S.empty[s], ((it / STAGES) & 1u) ^ 1u);
           S.st[s].hdr = f.h;
           if (f.h.flags & TILE_FAST) {
-            mbar_arrive_expect_tx(&S.full[s], f.nts * 2u + f.noff + f.nby);
-            bulk_g2s(S.st[s].ts, f.gts, f.nts, &S.full[s]);
-            bulk_g2s(S.st[s].val, f.gval, f.nts, &S.full[s]);
+            mbar_arrive_expect_tx(&S.full[s], f.nval + f.nts + f.noff + f.nby);
+            if (f.nts) bulk_g2s(S.st[s].ts, f.gts, f.nts, &S.full[s]);
+            bulk_g2s(S.st[s].val, f.gval, f.nval, &S.full[s]);
             bulk_g2s(S.st[s].off, f.goff, f.noff, &S.full[s]);
             if (f.nby) bulk_g2s(S.st[s].bytes, f.gby, f.nby, &S.full[s]);
           } else {
@@ -467,6 +472,7 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
   // hint stores into a few hundred hot dictionary sectors that every SM keeps reading bounce those lines between the two L2
   // partitions (ncu on cfg 1: 57 % of the samples waiting for the probe, LSU pipe 6 % busy)
   const bool use_hints = !(P.flags & AGG_NO_HINTS) && P.priv == nullptr, use_queue = !(P.flags & AGG_NO_QUEUE);
+  const bool scalar_probe = (P.flags & AGG_SCALAR_PROBE) != 0;
   uint32_t qcount = 0;                 // warp-uniform
   for (uint32_t it = 0;; it++) {
     const int s = it % STAGES;
@@ -509,10 +515,12 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
       const bool plain = mbase != nullptr && (bhi & 0x7FF00000u) != 0x7FF00000u && ((bhi << 1) | blo) != 0u;
       uint32_t gid = 0; uint64_t hint = 0;
       bool need_slow = live && (klen > (uint32_t)INLINE_KEY || keys_global), park = false, hit = false;
-      // ONE dictionary probe (32 B sector, carries the group's min/max hint)
-      if (live && !need_slow) {
-        uint64_t sa, sb, sc, sd;
-        ld_slot(slots + idx, sa, sb, sc, sd);
+      // ONE dictionary probe (32 B sector, carries the group's min/max hint), by lane pairs: one sector request per row
+      const bool probe = live && !need_slow;
+      uint64_t sa = 0, sb = 0, sc = 0, sd = 0;       // defined on every path: an undefined value would be carried over from the last tile
+      if (scalar_probe) { if (probe) ld_slot(slots + idx, sa, sb, sc, sd); }       // warp-uniform
+      else if (__any_sync(0xffffffffu, probe)) ld_slot_paired(slots, idx, (uint32_t)odd, sa, sb, sc, sd);
+      if (probe) {
         const uint32_t state = (uint32_t)(sd >> 32);
         if (state - 1u < 0xFFFFFFFEu && !slot_keys_unsettled(sa, sb)) {   // occupied and published (key words read after the insert)
           if ((uint32_t)sd == klen && (uint32_t)sa == w0 && (uint32_t)(sa >> 32) == w1 && (uint32_t)sb == w2 && (uint32_t)(sb >> 32) == w3) {
@@ -559,7 +567,7 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
           if (tmax >= hmax) red_max_u64(&mbase[gid].maxkey, ((unsigned long long)(ohi - 0x00100000u) << 32) | olo);
           pk = gid | (1u << 29);
         } else {
-          agg_apply_slow(P, H, r, st.ts[r], v, gid);
+          agg_apply_slow(P, st, r, v, gid);
         }
       }
       // count and sum by lane pairs: in each of two instructions lanes 2j / 2j+1 update {cnt, sum} of ONE row -- adjacent words of

@@ -150,7 +150,9 @@ struct AggParams {
   // k_merge_private folds into the pane afterwards (everything is commutative).  nullptr: disabled.
   GroupState* priv; uint32_t priv_groups;
 };
-enum : uint32_t { AGG_NO_HINTS = 1, AGG_NO_QUEUE = 2 };   // experiments: reduce min/max for every row; loop on collisions
+// experiments: reduce min/max for every row; loop on collisions; both slot halves loaded by the row's own lane; stage the
+// timestamps of every tile
+enum : uint32_t { AGG_NO_HINTS = 1, AGG_NO_QUEUE = 2, AGG_SCALAR_PROBE = 4, AGG_STAGE_TS = 8 };
 
 // ------------------------------------------------------------------------------------------------
 // Emission: combine the panes of one window, evaluate the predicate, compact into Arrow-shaped columns.

@@ -711,7 +711,8 @@ AggParams dnz_window::build_agg_params(Slot& s, const RunGeom& g, bool dirty, in
   CK(cudaMemsetAsync(&sc, 0, offsetof(SlotCtl, emit_blocked), stream));        // deferred-row counter, flags, tile counter (not the emit-blocked flag)
   P.batches = s.d_batches.as<BatchDesc>(); P.tiles = s.d_tiles.as<TileDesc>(); P.tile_begin = g.t0; P.tile_end = g.t1;
   P.dict = dict_view();
-  P.flags = ((cfg.flags & DNZ_FLAG_NO_HINTS) ? AGG_NO_HINTS : 0) | ((cfg.flags & DNZ_FLAG_NO_QUEUE) ? AGG_NO_QUEUE : 0);
+  P.flags = ((cfg.flags & DNZ_FLAG_NO_HINTS) ? AGG_NO_HINTS : 0) | ((cfg.flags & DNZ_FLAG_NO_QUEUE) ? AGG_NO_QUEUE : 0) |
+            ((cfg.flags & DNZ_FLAG_SCALAR_PROBE) ? AGG_SCALAR_PROBE : 0) | ((cfg.flags & DNZ_FLAG_STAGE_TS) ? AGG_STAGE_TS : 0);
   const size_t defer_cap = (size_t)std::max<int64_t>(g.rows, 1);
   s.d_defer[out_list].reserve(defer_cap * sizeof(DeferEntry));
   P.defer.entries = s.d_defer[out_list].as<DeferEntry>();

@@ -44,6 +44,8 @@ enum { DNZ_TS_CANONICAL = 0, DNZ_TS_INT64_MILLIS = 1, DNZ_TS_INT64_SECONDS = 2, 
 #define DNZ_FLAG_NO_PRIVATE 16u     /* experiments: no per-CTA private pane copies for low-cardinality streams        */
 #define DNZ_FLAG_NO_QUEUE 8u        /* experiments: colliding probes loop in place instead of using the retry queue */
 #define DNZ_FLAG_SYNCHRONOUS 32u    /* testing / A-B: wait for every aggregate launch before emitting (no speculative pipeline) */
+#define DNZ_FLAG_SCALAR_PROBE 64u   /* experiments: every row loads both halves of its dictionary slot (no lane-paired probe) */
+#define DNZ_FLAG_STAGE_TS 128u      /* experiments: stage the timestamps of tiles that lie inside one pane too              */
 
 typedef struct {
   int32_t kind;          /* DNZ_AGG_*                                            */
