@@ -30,6 +30,9 @@ FLAG_SYNCHRONOUS = 32
 FLAG_SCALAR_PROBE = 64
 FLAG_STAGE_TS = 128
 INTERNAL_METADATA_COLUMN = "_streaming_internal_metadata"   # crates/common/src/lib.rs:5
+SYNTH_SENSOR_KEYS, SYNTH_UUID_KEYS, SYNTH_INT64_KEYS = 0, 1, 2    # dnz_synth_generate key_kind
+# integer group-key types (Arrow formats l / i / L / I) -> numpy dtype of their values
+INT_KEY_DTYPES = {pa.int64(): np.int64, pa.int32(): np.int32, pa.uint64(): np.uint64, pa.uint32(): np.uint32}
 
 
 class DnzError(RuntimeError):
@@ -235,16 +238,19 @@ def make_record_batch(ts, val, key_off, key_bytes, ts_valid=None, val_valid=None
 
 
 class DeviceBatches:
-    """Synthetic sensor batches generated directly in device memory (dnz_synth_generate)."""
+    """Synthetic sensor batches generated directly in device memory (dnz_synth_generate).  int_keys: Int64 keys equal to the key
+    id (the ids of the "sensor_<id>" keys of the default stream), key_off = NULL."""
 
     def __init__(self, n_rows, batch_rows=65536, *, row0=0, seed=42, groups=1000, rows_per_ms=1000,
-                 t0_ms=1_700_000_000_000, uuid_keys=False, device=0, key_mul=1, key_add=0):
+                 t0_ms=1_700_000_000_000, uuid_keys=False, device=0, key_mul=1, key_add=0, int_keys=False):
+        assert not (uuid_keys and int_keys)
         L = lib()
         self.n_batches = (n_rows + batch_rows - 1) // batch_rows
         self.n_rows = n_rows
         self.array = (DeviceBatchC * self.n_batches)()
         self._arena = C.c_void_p()
-        rc = L.dnz_synth_generate(device, row0, n_rows, batch_rows, seed, groups, rows_per_ms, t0_ms, 1 if uuid_keys else 0,
+        kind = SYNTH_INT64_KEYS if int_keys else SYNTH_UUID_KEYS if uuid_keys else SYNTH_SENSOR_KEYS
+        rc = L.dnz_synth_generate(device, row0, n_rows, batch_rows, seed, groups, rows_per_ms, t0_ms, kind,
                                   key_mul, key_add, C.byref(self._arena), self.array, self.n_batches)
         if rc != 0:
             raise DnzError(rc, L.dnz_window_last_error(None).decode())
@@ -273,6 +279,7 @@ class GpuStreamingWindow:
         self._L = lib()
         self._h = C.c_void_p()
         names = schema.names
+        self._key_dtype = INT_KEY_DTYPES.get(schema.field(key).type) if key is not None else None   # None: Utf8 keys
         self._aliases = [a[2].encode() for a in aggs]
         arr = (_Agg * len(aggs))(*[_Agg(AGG_KINDS[k], names.index(col), al) for (k, col, _), al in zip(aggs, self._aliases)])
         ts_source, ts_column, ts_format = timestamp if timestamp else (0, 0, None)      # (TS_* kind, column name, chrono format)
@@ -330,7 +337,8 @@ class GpuStreamingWindow:
         return r
 
     def fetch_device_result(self, r: DeviceResultC, max_keys=None) -> dict:
-        """Copy a device-resident result to host arrays (test helper); keys are materialised for the first max_keys rows."""
+        """Copy a device-resident result to host arrays (test helper); keys are materialised for the first max_keys rows.
+        Integer keys (key_off == NULL): "key" holds Python ints (None for the NULL key) and "key_values" the value array."""
         n = r.n_rows
 
         def get(ptr, dt, m):
@@ -340,6 +348,16 @@ class GpuStreamingWindow:
                 if rc:
                     raise DnzError(rc, "memcpy")
             return a
+        if not r.key_off:
+            dt = np.dtype(self._key_dtype)
+            assert self._key_dtype is not None and r.key_bytes_len == n * dt.itemsize, "integer key result of another layout"
+            vals = get(r.key_bytes, dt, n)
+            kv = get(r.key_valid, np.uint8, n)
+            nk = n if max_keys is None else min(n, max_keys)
+            return {"key": [int(vals[i]) if kv[i] else None for i in range(nk)], "key_values": vals, "key_valid": kv,
+                    "count": get(r.count, np.int64, n), "min": get(r.min, np.float64, n), "max": get(r.max, np.float64, n),
+                    "avg": get(r.avg, np.float64, n), "sum": get(r.sum, np.float64, n), "agg_valid": get(r.agg_valid, np.uint8, n),
+                    "window_start": get(r.window_start_ms, np.int64, n), "window_end": get(r.window_end_ms, np.int64, n)}
         off = np.concatenate([get(r.key_off, np.int32, n), np.array([r.key_bytes_len], np.int32)])
         kb_arr = get(r.key_bytes, np.uint8, r.key_bytes_len)
         kb = kb_arr.tobytes() if (max_keys is None or max_keys > 0) else b""

@@ -166,6 +166,7 @@ class StreamingWindowExec {
     for (auto& a : aggr_) aggs.push_back(dnz_agg{a.kind, col_index(a.arg_column), a.alias.c_str()});
     dnz_window_config c{};
     c.abi_version = DNZ_ABI_VERSION; c.device = device_;
+    // the group key column: Utf8, Int64, Int32, UInt64 or UInt32 (the library returns DNZ_ERR_UNSUPPORTED for any other type)
     c.key_column = group_by_.columns.empty() ? DNZ_NO_KEY : col_index(group_by_.columns[0]);      // `.window([], ..)`: WindowAggStream
     if (timestamp_unit_.source != DNZ_TS_CANONICAL) {
       c.ts_source = timestamp_unit_.source; c.ts_column = col_index(timestamp_column_);

@@ -143,6 +143,26 @@ struct KeyRef {
   const uint8_t* ptr;    // original bytes (needed only for long keys)
 };
 
+// Stored form of an integer key (Arrow Int64 / Int32 / UInt64 / UInt32) of `width` bytes (4 or 8): k0 = the value's bits,
+// zero-extended; k1 = INT_KEY_TAG; len = width.  An ordinary inline key from then on (hash, owner, placement, checkpoint, the
+// pack kernel's key bytes).  The tag keeps the key words non-zero: all-zero key words are the probe's torn-read marker
+// (slot_keys_unsettled), and with k1 = 0 every row of the key 0 would take the ordered reload and the full lookup.
+// Every builder of an integer key goes through int_key, so one value can never become two groups.
+constexpr uint64_t INT_KEY_TAG = 0x494E544B45594B31ull;    // "1KYEKTNI": any non-zero constant
+__host__ __device__ __forceinline__ KeyRef int_key(uint64_t bits, uint32_t width) {
+  KeyRef k;
+  k.k0 = width == 4u ? (uint64_t)(uint32_t)bits : bits; k.k1 = INT_KEY_TAG; k.len = width; k.ptr = nullptr;
+  k.hash = hash_inline(k.k0, k.k1, width);
+  return k;
+}
+// the integer key of row `row` of a values buffer (naturally aligned: the host copy is, device batches are checked)
+template <int KW>
+__device__ __forceinline__ KeyRef load_int_key(const uint8_t* values, int64_t row) {
+  static_assert(KW == 4 || KW == 8, "integer key width");
+  if (KW == 8) return int_key((uint64_t)__ldg(reinterpret_cast<const unsigned long long*>(values) + row), 8u);
+  return int_key((uint64_t)__ldg(reinterpret_cast<const uint32_t*>(values) + row), 4u);
+}
+
 // Load up to 16 key bytes from an arbitrarily aligned address using aligned 32-bit loads.
 // Reading the aligned words that contain the first / last key byte never leaves their 4 B word, so it is
 // safe for both shared and global memory.

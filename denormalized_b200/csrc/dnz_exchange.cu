@@ -51,7 +51,7 @@ __device__ __forceinline__ PartialEntry pack_entry(const PackParams& P, int j, u
   PartialEntry e;
   e.pane = P.pane[j]; e.cnt = (unsigned long long)s.cnt; e.sum = s.sum; e.minkey = s.minkey; e.maxkey = s.maxkey;
   e.nullrows = P.nullrows[j] ? P.nullrows[j][g] : 0ull; e.fz = P.fz[j] ? P.fz[j][g] : ~0ull;
-  e.key_off = key_off; e.key_len = c.null_key ? 0xFFFFFFFFu : c.klen;
+  e.key_off = key_off; e.key_len = c.null_key ? 0xFFFFFFFFu : (c.klen | P.key_tag);
   return e;
 }
 // A 64 B packet leaves as four 128-bit stores, the widest store sm_90 has (a peer write travels NVLink per store instruction).
@@ -95,11 +95,17 @@ cudaError_t launch_pack_partials(const PackParams& p, cudaStream_t s) {
 }
 
 // ---- merge: thread per received packet ---------------------------------------------------------------------------------
-// Intern the packet's key (its bytes at `key`) and fold its partial state into the main pane it names.
+// Intern the packet's key (its bytes at `key`, 8 B aligned) and fold its partial state into the main pane it names.  Integer keys
+// are rebuilt with int_key from the value the pack kernel wrote (the low key_width bytes of the stored k0).  A packet of another
+// key type (its key_len carries the sender's type above KEY_TYPE_SHIFT) raises error bit 8 and is not merged.
 __device__ __forceinline__ void merge_packet(const MergeParams& P, const PartialEntry& e, const uint8_t* key) {
   uint32_t gid;
   if (e.key_len == 0xFFFFFFFFu) gid = dict_lookup_null(P.dict);
-  else {
+  else if ((e.key_len >> KEY_TYPE_SHIFT) != (P.key_tag >> KEY_TYPE_SHIFT)) { atomicOr(P.error, 8u); return; }
+  else if (P.key_width != 0) {
+    if (e.key_len != (P.key_tag | (uint32_t)P.key_width)) { atomicOr(P.error, 8u); return; }
+    gid = dict_lookup(P.dict, P.key_width == 8 ? load_int_key<8>(key, 0) : load_int_key<4>(key, 0), false);
+  } else {
     KeyRef k; load_key<false>(key, e.key_len, k);
     gid = dict_lookup(P.dict, k, false);
   }

@@ -43,7 +43,7 @@ void dnz_window::export_partials(int64_t watermark, dnz_partials* out) {
   d_owner_cursor.reserve((size_t)world * 8); d_pack_dest.reserve((size_t)world * sizeof(PackDest));
   h_small.reserve((size_t)std::max<size_t>(256, world * sizeof(PackDest)));
   PackParams P; memset(&P, 0, sizeof P);
-  P.n_groups = n_groups_host; P.rank = rank; P.world = world; P.dict = dict_view();
+  P.n_groups = n_groups_host; P.rank = rank; P.world = world; P.dict = dict_view(); P.key_tag = key_tag();
   P.owner_cursor = d_owner_cursor.as<unsigned long long>(); P.dest = d_pack_dest.as<PackDest>();
   auto run_pass = [&](int pass) {
     CK(cudaMemsetAsync(d_owner_cursor.p, 0, (size_t)world * 8, stream));
@@ -98,11 +98,12 @@ void dnz_window::import_partials(const uint8_t* entries, const int64_t* src_coun
   h_xptrs.reserve(7 * pb); d_xptrs.reserve(7 * pb);
   M.panes = upload_pane_table(h_xptrs.as<void*>(), d_xptrs.as<char>(), pane_lo, pane_hi, [&](int64_t p) { return std::make_pair(get_pane(p, false), (Pane*)nullptr); });
   CK(cudaMemsetAsync(&ctl()->merge_err, 0, 4, stream));
-  M.entries = reinterpret_cast<const PartialEntry*>(entries); M.n_entries = n; M.key_bytes = key_bytes; M.world = world;
+  M.entries = reinterpret_cast<const PartialEntry*>(entries); M.n_entries = n; M.key_bytes = key_bytes; M.world = world; M.key_width = key_width; M.key_tag = key_tag();
   M.dict = dict_view(); M.error = &ctl()->merge_err;
   CK(launch_merge_partials(M, stream)); stats.total_launches++;
   fetch_ctl();
   uint32_t err = h_small.as<CtlBlock>()->merge_err;
+  if (err & 8u) fail(DNZ_ERR_INVALID, "pane exchange: the packets hold keys of another type than this operator's group key (every rank must group by the same key type)");
   if (err) fail(DNZ_ERR_NOMEM, "pane merge failed (flags %u): table sizing error", err);
   stats.exchanged_in += n;
 }
@@ -301,7 +302,7 @@ void dnz_window::group_pack(dnz_group* g) {
   g->tmark(0, stream);
   CK(cudaMemsetAsync(g->d_owner_cursor.p, 0, MAX_WORLD * 8, stream));
   PackParams P; memset(&P, 0, sizeof P);
-  P.n_groups = gcap; P.rank = rank; P.world = world; P.dict = dict_view();      // grid bound; the kernels clamp to the device counter
+  P.n_groups = gcap; P.rank = rank; P.world = world; P.dict = dict_view(); P.key_tag = key_tag();      // grid bound; the kernels clamp to the device counter
   P.owner_cursor = g->d_owner_cursor.as<unsigned long long>(); P.dest = g->d_pack_dest.as<PackDest>();
   auto pack = [&] { CK(launch_pack_partials(P, stream)); stats.total_launches++; };
   P.pass = 0;
@@ -344,7 +345,7 @@ void dnz_window::group_finish(dnz_group* g, int64_t* gwm_out) {
       MergeParams M; memset(&M, 0, sizeof M);
       M.panes = upload_pane_table(reinterpret_cast<void**>(h_xptrs.as<char>() + (size_t)mp * half_bytes), d_xptrs.as<char>() + (size_t)mp * half_bytes,
                                   gfirst, hi, [&](int64_t p) { return std::make_pair(get_pane(p, false), (Pane*)nullptr); });
-      M.world = world; M.dict = dict_view(); M.error = &ctl()->merge_err;
+      M.world = world; M.key_width = key_width; M.key_tag = key_tag(); M.dict = dict_view(); M.error = &ctl()->merge_err;
       CK(launch_merge_ring(M, X, g->d_totals.as<unsigned long long>() + 1, sm_count, stream)); stats.total_launches++;
     }
     CK(cudaMemsetAsync(&g->view.self.ctl->cursor[mp], 0, 8, stream));       // the ring half is free again ...

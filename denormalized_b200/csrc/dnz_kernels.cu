@@ -189,7 +189,9 @@ __device__ __forceinline__ bool apply_row(const AggParams& P, uint32_t tile, uin
   return true;
 }
 
-// One row read straight from global memory (bitmaps honoured).
+// One row read straight from global memory (bitmaps honoured).  KW: key width, 0 = Utf8 (offsets + bytes), 4 / 8 = integer
+// keys (BatchDesc::bytes holds the values, one per row).
+template <int KW>
 __device__ __forceinline__ void process_row_generic(const AggParams& P, uint32_t tile, const TileDesc& td, const BatchDesc& bd,
                                                     uint32_t r) {
   int64_t row = (int64_t)td.row0 + r;
@@ -200,9 +202,13 @@ __device__ __forceinline__ void process_row_generic(const AggParams& P, uint32_t
   bool key_ok = !bd.key_valid || bit_at(bd.key_valid, bd.key_vbit + row);
   uint32_t gid;
   if (key_ok) {
-    int32_t o0 = bd.off[row], o1 = bd.off[row + 1];
-    KeyRef k; load_key<false>(bd.bytes + o0, (uint32_t)(o1 - o0), k);
-    gid = dict_lookup(P.dict, k, false);
+    if constexpr (KW == 0) {
+      int32_t o0 = bd.off[row], o1 = bd.off[row + 1];
+      KeyRef k; load_key<false>(bd.bytes + o0, (uint32_t)(o1 - o0), k);
+      gid = dict_lookup(P.dict, k, false);
+    } else {
+      gid = dict_lookup(P.dict, load_int_key<KW>(bd.bytes, row), false);
+    }
   } else gid = dict_lookup_null(P.dict);
   if (gid == GID_DEFER_GROUPS) { defer_row(P.defer, tile, r, DEFER_GROUPS_FULL); return; }
   if (gid == GID_DEFER_ARENA) { defer_row(P.defer, tile, r, DEFER_ARENA_FULL); return; }
@@ -211,21 +217,23 @@ __device__ __forceinline__ void process_row_generic(const AggParams& P, uint32_t
   apply_row(P, tile, r, pane, val_ok, v, gid, rowseq);
 }
 
+template <int KW>
 __global__ void __launch_bounds__(256) k_aggregate_generic(const __grid_constant__ AggParams P) {
   for (int64_t t = P.tile_begin + blockIdx.x; t < P.tile_end; t += gridDim.x) {
     const TileDesc td = P.tiles[t];
     if (td.flags & TILE_EMPTY) continue;
     const BatchDesc bd = P.batches[td.batch];
-    for (uint32_t r = threadIdx.x; r < (uint32_t)td.n_rows; r += blockDim.x) process_row_generic(P, (uint32_t)(t - P.tile_begin), td, bd, r);
+    for (uint32_t r = threadIdx.x; r < (uint32_t)td.n_rows; r += blockDim.x) process_row_generic<KW>(P, (uint32_t)(t - P.tile_begin), td, bd, r);
   }
 }
 
+template <int KW>
 __global__ void __launch_bounds__(256) k_deferred(const __grid_constant__ AggParams P, uint64_t n_entries, const DeferEntry* entries) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_entries; i += (uint64_t)gridDim.x * blockDim.x) {
     DeferEntry e = entries[i];
     const TileDesc td = P.tiles[P.tile_begin + e.tile];
     const BatchDesc bd = P.batches[td.batch];
-    process_row_generic(P, e.tile, td, bd, e.row);
+    process_row_generic<KW>(P, e.tile, td, bd, e.row);
   }
 }
 
@@ -320,11 +328,12 @@ __device__ __noinline__ uint64_t agg_probe_words(const AggParams& P, uint4 kw, u
   uint32_t slot = 0; uint32_t g = dict_lookup(P.dict, k, false, &slot);
   return ((uint64_t)slot << 32) | g;
 }
+template <int KW>
 __device__ __noinline__ void agg_tile_generic(const AggParams& P, uint32_t tile_rel, int tid) {
   const TileDesc td = P.tiles[P.tile_begin + tile_rel];
   if (td.flags & TILE_EMPTY) return;
   const BatchDesc bd = P.batches[td.batch];
-  for (uint32_t r = tid; r < (uint32_t)td.n_rows; r += CONSUMER_WARPS * 32) process_row_generic(P, tile_rel, td, bd, r);
+  for (uint32_t r = tid; r < (uint32_t)td.n_rows; r += CONSUMER_WARPS * 32) process_row_generic<KW>(P, tile_rel, td, bd, r);
 }
 
 // One full-warp probe round over the top (up to) 32 parked rows.  Rows that resolve are accumulated with scalar
@@ -376,7 +385,13 @@ __device__ __noinline__ uint32_t agg_queue_round(const AggParams& P, WarpQueue& 
   return base + __popc(bal);
 }
 
+// KW: key width.  0 = Utf8 (offsets + key bytes staged, 4-5 LDS.32 + funnel shifts per key); 4 / 8 = integer keys: the tile's
+// values are staged as the key bytes (one copy of n_rows x KW bytes, no offsets), a key is one or two LDS.32 plus int_key's
+// constant tag words.  Everything from the hash on is the same code.
+template <int KW>
 __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_constant__ AggParams P) {
+  static_assert(KW == 0 || KW == 4 || KW == 8, "key width");
+  static_assert(KW * TILE <= BCAP, "a tile's integer keys fit the key stage");
   extern __shared__ __align__(128) uint8_t smem_raw[];
   AggSmem& S = *reinterpret_cast<AggSmem*>(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -406,6 +421,10 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
           d.nval = round16((uint32_t)td.n_rows * 8u); d.noff = round16(((uint32_t)td.n_rows + 1u) * 4u);
           d.nts = ((td.flags & TILE_PANE_UNIFORM) && !(P.flags & AGG_STAGE_TS)) ? 0u : d.nval;
           d.nby = (td.flags & TILE_KEYS_GLOBAL) ? 0u : round16((uint32_t)(td.byte0 + td.byte_len - h.a0));
+          if constexpr (KW != 0) {                       // integer keys: the tile's values are its key bytes, no offsets
+            d.goff = nullptr; d.noff = 0u;
+            d.gby = bd.bytes + (size_t)td.row0 * KW; d.nby = round16((uint32_t)td.n_rows * KW);
+          }
           h.gbytes = bd.bytes;
           if (td.flags & TILE_PANE_UNIFORM) {
             int64_t pi = td.pane_lo - P.panes.pane0;
@@ -446,7 +465,7 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
             mbar_arrive_expect_tx(&S.full[s], f.nval + f.nts + f.noff + f.nby);
             if (f.nts) bulk_g2s(S.st[s].ts, f.gts, f.nts, &S.full[s]);
             bulk_g2s(S.st[s].val, f.gval, f.nval, &S.full[s]);
-            bulk_g2s(S.st[s].off, f.goff, f.noff, &S.full[s]);
+            if constexpr (KW == 0) bulk_g2s(S.st[s].off, f.goff, f.noff, &S.full[s]);
             if (f.nby) bulk_g2s(S.st[s].bytes, f.gby, f.nby, &S.full[s]);
           } else {
             mbar_arrive(&S.full[s]);
@@ -488,28 +507,38 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
     const int lane = (int)(tix & 31u), odd = (int)(tix & 1u);
     WarpQueue& Q = S.q[tix >> 5];
     if (!(h0.y & TILE_FAST)) {
-      agg_tile_generic(P, H.tile_rel, (int)tix);
+      agg_tile_generic<KW>(P, H.tile_rel, (int)tix);
     } else {
       const uint4 h1 = *reinterpret_cast<const uint4*>(&H.mbase);         // mbase, tile_rel, pane_rel
       const uint32_t r = tix;
       const bool live = r < (uint32_t)h0.x;
       GroupState* const mbase = reinterpret_cast<GroupState*>(((uint64_t)h1.y << 32) | h1.x);
       const double v = st.val[r];
-      const int32_t o0 = st.off[r], o1 = st.off[r + 1];
-      const bool keys_global = (h0.y & TILE_KEYS_GLOBAL) != 0;          // warp-uniform: the key bytes were not staged
-      const uint32_t klen = live ? (uint32_t)(o1 - o0) : 0u, kb = (live && !keys_global) ? (uint32_t)(o0 - h0.z) : 0u;
-      const uint32_t addr = smem_u32(st.bytes) + kb, q = addr & ~3u, mis = addr & 3u, sh = mis * 8u;
-      uint32_t a[5];
+      const int32_t o0 = KW == 0 ? st.off[r] : 0, o1 = KW == 0 ? st.off[r + 1] : 0;
+      const bool keys_global = KW == 0 && (h0.y & TILE_KEYS_GLOBAL) != 0;   // warp-uniform: the key bytes were not staged
+      const uint32_t klen = KW != 0 ? (uint32_t)KW : live ? (uint32_t)(o1 - o0) : 0u, kb = (live && !keys_global) ? (uint32_t)(o0 - h0.z) : 0u;
+      uint32_t w0, w1, w2, w3, idx;
+      if constexpr (KW == 0) {                     // Utf8: offsets + up to 16 staged key bytes
+        const uint32_t addr = smem_u32(st.bytes) + kb, q = addr & ~3u, mis = addr & 3u, sh = mis * 8u;
+        uint32_t a[5];
 #pragma unroll
-      for (int j = 0; j < 4; j++) a[j] = lds32(q + 4u * j);
-      a[4] = (mis + klen > 16u) ? lds32(q + 16u) : 0u;                    // a 5th word only when the key straddles it
-      // byte mask of word i of a klen-byte key: 0xFFFFFFFF >> clamp(32 - 8 * (klen - 4 i), 0, 32)  (shf.r.clamp saturates at 32)
-      const int mb = 32 - 8 * (int)min(klen, (uint32_t)INLINE_KEY);
-      const uint32_t w0 = __funnelshift_r(a[0], a[1], sh) & __funnelshift_rc(0xFFFFFFFFu, 0u, (uint32_t)max(mb, 0));
-      const uint32_t w1 = __funnelshift_r(a[1], a[2], sh) & __funnelshift_rc(0xFFFFFFFFu, 0u, (uint32_t)max(mb + 32, 0));
-      const uint32_t w2 = __funnelshift_r(a[2], a[3], sh) & __funnelshift_rc(0xFFFFFFFFu, 0u, (uint32_t)max(mb + 64, 0));
-      const uint32_t w3 = __funnelshift_r(a[3], a[4], sh) & __funnelshift_rc(0xFFFFFFFFu, 0u, (uint32_t)max(mb + 96, 0));
-      uint32_t idx = hash_words(w0, w1, w2, w3, klen) & dmask;
+        for (int j = 0; j < 4; j++) a[j] = lds32(q + 4u * j);
+        a[4] = (mis + klen > 16u) ? lds32(q + 16u) : 0u;                    // a 5th word only when the key straddles it
+        // byte mask of word i of a klen-byte key: 0xFFFFFFFF >> clamp(32 - 8 * (klen - 4 i), 0, 32)  (shf.r.clamp saturates at 32)
+        const int mb = 32 - 8 * (int)min(klen, (uint32_t)INLINE_KEY);
+        w0 = __funnelshift_r(a[0], a[1], sh) & __funnelshift_rc(0xFFFFFFFFu, 0u, (uint32_t)max(mb, 0));
+        w1 = __funnelshift_r(a[1], a[2], sh) & __funnelshift_rc(0xFFFFFFFFu, 0u, (uint32_t)max(mb + 32, 0));
+        w2 = __funnelshift_r(a[2], a[3], sh) & __funnelshift_rc(0xFFFFFFFFu, 0u, (uint32_t)max(mb + 64, 0));
+        w3 = __funnelshift_r(a[3], a[4], sh) & __funnelshift_rc(0xFFFFFFFFu, 0u, (uint32_t)max(mb + 96, 0));
+        idx = hash_words(w0, w1, w2, w3, klen) & dmask;
+      } else {
+        // the stored form of int_key: value bits in w0 / w1, the tag (compile-time constants) in w2 / w3
+        const uint32_t addr = smem_u32(st.bytes) + r * (uint32_t)KW;
+        const uint32_t lo = lds32(addr), hi = KW == 8 ? lds32(addr + 4u) : 0u;
+        const KeyRef k = int_key(((uint64_t)hi << 32) | lo, (uint32_t)KW);
+        w0 = (uint32_t)k.k0; w1 = (uint32_t)(k.k0 >> 32); w2 = (uint32_t)k.k1; w3 = (uint32_t)(k.k1 >> 32);
+        idx = (uint32_t)k.hash & dmask;
+      }
       // paired-path row: finite and not +-0.0 (everything else goes through the general per-row path)
       const uint32_t bhi = (uint32_t)__double2hiint(v), blo = (uint32_t)__double2loint(v);
       const bool plain = mbase != nullptr && (bhi & 0x7FF00000u) != 0x7FF00000u && ((bhi << 1) | blo) != 0u;
@@ -541,7 +570,9 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
         qcount += __popc(bal);
       }
       if (need_slow) {
-        const uint64_t gs = keys_global ? agg_probe_slow_global(P, H.gbytes + o0, klen) : agg_probe_slow(P, st.bytes + kb, klen);
+        uint64_t gs;
+        if constexpr (KW == 0) gs = keys_global ? agg_probe_slow_global(P, H.gbytes + o0, klen) : agg_probe_slow(P, st.bytes + kb, klen);
+        else gs = agg_probe_words(P, make_uint4(w0, w1, w2, w3), klen);
         gid = (uint32_t)gs; idx = (uint32_t)(gs >> 32); hint = 0; hit = true;
       }
       uint32_t pk = 0;
@@ -597,17 +628,24 @@ __global__ void __launch_bounds__(AGG_THREADS, 2) k_aggregate(const __grid_const
 static int g_agg_smem = 0;
 cudaError_t agg_kernel_setup() {
   g_agg_smem = (int)sizeof(AggSmem);
-  return cudaFuncSetAttribute(k_aggregate, cudaFuncAttributeMaxDynamicSharedMemorySize, g_agg_smem);
+  for (auto k : {k_aggregate<0>, k_aggregate<4>, k_aggregate<8>}) {
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, g_agg_smem);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 int aggregate_grid(int64_t n_tiles, int sm_count) {
   return (int)(n_tiles < (int64_t)sm_count * 2 ? n_tiles : (int64_t)sm_count * 2);          // two persistent CTAs per SM
 }
-cudaError_t launch_aggregate(const AggParams& p, int sm_count, cudaStream_t s) {
+cudaError_t launch_aggregate(const AggParams& p, int key_width, int sm_count, cudaStream_t s) {
   int64_t n_tiles = p.tile_end - p.tile_begin;
   if (n_tiles <= 0) return cudaSuccess;
   if (!g_agg_smem) { cudaError_t e = agg_kernel_setup(); if (e != cudaSuccess) return e; }
-  k_aggregate<<<aggregate_grid(n_tiles, sm_count), AGG_THREADS, g_agg_smem, s>>>(p);
+  const dim3 grid(aggregate_grid(n_tiles, sm_count));
+  if (key_width == 8) k_aggregate<8><<<grid, AGG_THREADS, g_agg_smem, s>>>(p);
+  else if (key_width == 4) k_aggregate<4><<<grid, AGG_THREADS, g_agg_smem, s>>>(p);
+  else k_aggregate<0><<<grid, AGG_THREADS, g_agg_smem, s>>>(p);
   return cudaGetLastError();
 }
 
@@ -632,16 +670,21 @@ cudaError_t launch_merge_private(const AggParams& p, int grid, cudaStream_t s) {
   k_merge_private<<<g, 256, 0, s>>>(p, grid);
   return cudaGetLastError();
 }
-cudaError_t launch_aggregate_generic(const AggParams& p, int sm_count, cudaStream_t s) {
+cudaError_t launch_aggregate_generic(const AggParams& p, int key_width, int sm_count, cudaStream_t s) {
   int64_t n_tiles = p.tile_end - p.tile_begin;
   if (n_tiles <= 0) return cudaSuccess;
   int grid = (int)(n_tiles < (int64_t)sm_count * 8 ? n_tiles : (int64_t)sm_count * 8);
-  k_aggregate_generic<<<grid, 256, 0, s>>>(p);
+  if (key_width == 8) k_aggregate_generic<8><<<grid, 256, 0, s>>>(p);
+  else if (key_width == 4) k_aggregate_generic<4><<<grid, 256, 0, s>>>(p);
+  else k_aggregate_generic<0><<<grid, 256, 0, s>>>(p);
   return cudaGetLastError();
 }
-cudaError_t launch_deferred(const AggParams& p, const DeferEntry* in, uint64_t n_entries, cudaStream_t s) {
+cudaError_t launch_deferred(const AggParams& p, int key_width, const DeferEntry* in, uint64_t n_entries, cudaStream_t s) {
   if (!n_entries) return cudaSuccess;
-  k_deferred<<<stride_grid(n_entries, 8), 256, 0, s>>>(p, n_entries, in);
+  const unsigned grid = stride_grid(n_entries, 8);
+  if (key_width == 8) k_deferred<8><<<grid, 256, 0, s>>>(p, n_entries, in);
+  else if (key_width == 4) k_deferred<4><<<grid, 256, 0, s>>>(p, n_entries, in);
+  else k_deferred<0><<<grid, 256, 0, s>>>(p, n_entries, in);
   return cudaGetLastError();
 }
 
@@ -795,7 +838,7 @@ __global__ void __launch_bounds__(256) k_emit(const __grid_constant__ EmitParams
     c = combine_panes(P, g);
     if (c.present) {
       gk = P.dict.gid_key[g];
-      klen = gk.len == 0xFFFFFFFFu ? 0u : gk.len;
+      klen = gk.len == 0xFFFFFFFFu ? (uint32_t)P.key_width : gk.len;
       keep = P.world <= 1 || key_owner(gk, P.world) == P.rank;
       agg_ok = c.cnt != 0;
       if (agg_ok) {

@@ -173,6 +173,7 @@ struct EmitParams {
   double filter_lit;
   int64_t wstart, wend;
   uint32_t n_groups;             // upper bound (grid size); the kernel clamps to the device counter
+  int32_t key_width;             // 0: Utf8 keys; 4 / 8: integer keys, every row (the NULL key too) emits key_width bytes
   int32_t rank, world;           // multi-GPU: emit only keys with hash64 % world == rank (world <= 1: all)
   // speculative pipeline: gate[0 .. PIPELINE_SLOTS) are the control block's pipeline slots (nullptr: not gated).  While any
   // of their deferred-row counters is non-zero some rows of an earlier launch have not been applied yet: the launch does
@@ -188,9 +189,17 @@ struct __align__(16) PartialEntry {
   int64_t pane;
   unsigned long long cnt; double sum; unsigned long long minkey, maxkey;
   unsigned long long nullrows, fz;
-  uint32_t key_off, key_len;     // bytes at key_off inside the sender's key segment FOR THIS OWNER; key_len == 0xFFFFFFFF: NULL key
+  uint32_t key_off, key_len;     // bytes at key_off inside the sender's key segment FOR THIS OWNER; key_len == 0xFFFFFFFF: NULL key,
+                                 // integer keys: width | key type << KEY_TYPE_SHIFT (below)
 };
 static_assert(sizeof(PartialEntry) == 64, "packet size");
+// Group-key types: index = key type code (0 Utf8, 1 Int64, 2 Int32, 3 UInt64, 4 UInt32), the code a checkpoint records.  A packet
+// of an integer key carries key_len = width | code << KEY_TYPE_SHIFT, so that the owner's merge detects a rank that groups by
+// another key type; Utf8 packets carry the plain length (keys of 256 MiB or more are refused by the merge).
+struct KeyType { const char* format; int32_t width; };           // format: the Arrow C format string (a literal)
+constexpr KeyType KEY_TYPES[] = {{"u", 0}, {"l", 8}, {"i", 4}, {"L", 8}, {"I", 4}};
+constexpr int N_KEY_TYPES = 5;
+constexpr int KEY_TYPE_SHIFT = 28;
 constexpr int MAX_WORLD = 32;
 constexpr int PACK_PANES = 32;       // panes per pack launch (a 32-bit mask per group id)
 // Where the write pass puts one owner's packets and key bytes: its segment of the local export buffers, or its reserved range
@@ -206,10 +215,13 @@ struct PackParams {
   unsigned long long* owner_cursor;              // [world] (entries << 32) | key bytes, running over all launches of a pass
   const PackDest* dest;                          // [world] write pass: every owner's destination
   int32_t pass;                                  // 0: count, 1: write
+  uint32_t key_tag;                              // key type code << KEY_TYPE_SHIFT, or'ed into key_len (0: Utf8)
 };
 struct MergeParams {
   const PartialEntry* entries; int64_t n_entries; const uint8_t* key_bytes;
   int32_t world;
+  int32_t key_width;                             // 0: Utf8 keys; 4 / 8: integer keys (a packet's key bytes are the value, int_key)
+  uint32_t key_tag;                              // what a packet of this key type carries above KEY_TYPE_SHIFT in key_len
   int64_t src_entry_end[MAX_WORLD];              // prefix sums over the sending ranks
   int64_t src_key_base[MAX_WORLD];
   DictView dict; PaneTable panes;
@@ -220,16 +232,17 @@ struct MergeParams {
 // launch wrappers (dnz_kernels.cu)
 cudaError_t launch_tile_scan(const BatchDesc* batches, int64_t n_batches, int64_t n_tiles, int64_t pane_ms,
                              TileDesc* tiles, BatchMinMax* minmax, bool allow_fast, cudaStream_t s);
-cudaError_t launch_aggregate(const AggParams& p, int sm_count, cudaStream_t s);
+// key_width: 0 = Utf8 keys, 4 / 8 = integer keys (the instantiation of the kernel that matches the stream)
+cudaError_t launch_aggregate(const AggParams& p, int key_width, int sm_count, cudaStream_t s);
 int aggregate_grid(int64_t n_tiles, int sm_count);
 cudaError_t launch_merge_private(const AggParams& p, int grid, cudaStream_t s);
-cudaError_t launch_aggregate_generic(const AggParams& p, int sm_count, cudaStream_t s);
+cudaError_t launch_aggregate_generic(const AggParams& p, int key_width, int sm_count, cudaStream_t s);
 cudaError_t launch_aggregate_ungrouped(const AggParams& p, int sm_count, cudaStream_t s);
 // ungrouped windows: the panes of one closed window -> one partial state (read back by the host-side Final stage)
 struct UWindow { const GroupState* st[MAX_WINDOW_PANES]; const unsigned long long* nr[MAX_WINDOW_PANES]; int32_t n, pad; };
 struct UState { unsigned long long cnt; double sum; unsigned long long mink, maxk, nulls; };
 cudaError_t launch_ungrouped_collect(const UWindow* wins, int n, UState* out, cudaStream_t s);
-cudaError_t launch_deferred(const AggParams& p, const DeferEntry* in, uint64_t n_entries, cudaStream_t s);
+cudaError_t launch_deferred(const AggParams& p, int key_width, const DeferEntry* in, uint64_t n_entries, cudaStream_t s);
 cudaError_t launch_emit(const EmitParams& p, cudaStream_t s);
 cudaError_t launch_dict_rehash(const DictSlot* old_slots, uint32_t old_cap, DictView nd, cudaStream_t s);
 cudaError_t launch_clear_hints(DictSlot* slots, uint32_t cap, cudaStream_t s);
@@ -270,7 +283,7 @@ bool ts_format_supported(const char* fmt);
 
 // synthetic generator (dnz_synth.cu)
 cudaError_t launch_synth(int64_t row0, int64_t n_rows, int64_t batch_rows, uint64_t seed, int64_t groups,
-                         int64_t rows_per_ms, int64_t t0_ms, int uuid_keys, int64_t key_mul, int64_t key_add, int64_t* ts, double* val, int32_t* off,
+                         int64_t rows_per_ms, int64_t t0_ms, int key_kind, int64_t key_mul, int64_t key_add, int64_t* ts, double* val, int32_t* off,
                          uint8_t* bytes, int64_t bytes_stride, cudaStream_t s);
 
 }  // namespace dnz

@@ -96,7 +96,8 @@ void dnz_window::fill_schema(ArrowSchema* schema) {
     c->format = fmt; c->flags = flags; c->release = release_child_schema;
     sp->children.push_back(std::move(c));
   };
-  if (!ungrouped) add(key_name, "u", ARROW_FLAG_NULLABLE);
+  // the input's key type (a literal: the schema outlives the operator); integer keys keep the input field's nullability
+  if (!ungrouped) add(key_name, KEY_TYPES[key_type].format, (key_width == 0 || key_nullable) ? ARROW_FLAG_NULLABLE : 0);
   for (size_t i = 0; i < aggs.size(); i++) add(aliases[i], agg_format(aggs[i].kind), aggs[i].kind == DNZ_AGG_COUNT ? 0 : ARROW_FLAG_NULLABLE);
   add("window_start_time", "tsm:", 0);     // continuous/mod.rs:42-62: Timestamp(ms, None), non-null
   add("window_end_time", "tsm:", 0);
@@ -166,7 +167,8 @@ void dnz_window::export_arrow(ArrowArray* out, ArrowSchema* schema, int32_t* has
     }
     return h;
   };
-  int32_t* koff = (int32_t*)fetch(&ResultSet::key_off, 4, false, 4);
+  // integer keys: key_bytes holds key_width bytes per row, the Arrow values buffer itself (no offsets)
+  int32_t* koff = key_width ? nullptr : (int32_t*)fetch(&ResultSet::key_off, 4, false, 4);
   uint8_t* kbytes = (uint8_t*)fetch(&ResultSet::key_bytes, 1, true, 0);
   uint8_t* kvalid = (uint8_t*)fetch(&ResultSet::key_valid, 1, false, 0);
   int64_t* count = (int64_t*)fetch(&ResultSet::count, 8, false, 0);
@@ -175,7 +177,7 @@ void dnz_window::export_arrow(ArrowArray* out, ArrowSchema* schema, int32_t* has
   uint8_t* avalid = (uint8_t*)fetch(&ResultSet::agg_valid, 1, false, 0);
   int64_t* ws = (int64_t*)fetch(&ResultSet::wstart, 8, false, 0); int64_t* we = (int64_t*)fetch(&ResultSet::wend, 8, false, 0);
   CK(cudaStreamSynchronize(d2h_stream));
-  {   // key offsets are relative to each set's byte buffer: rebase them onto the concatenated export
+  if (koff) {   // key offsets are relative to each set's byte buffer: rebase them onto the concatenated export
     uint64_t row_at = 0, byte_at = 0;
     for (auto& g : ranges) {
       const int64_t delta = (int64_t)byte_at - (int64_t)g.b0;
@@ -183,7 +185,7 @@ void dnz_window::export_arrow(ArrowArray* out, ArrowSchema* schema, int32_t* has
       row_at += g.r1 - g.r0; byte_at += g.b1 - g.b0;
     }
   }
-  koff[n] = (int32_t)nbytes;
+  if (koff) koff[n] = (int32_t)nbytes;
   // byte-per-row validity -> Arrow bitmaps
   auto pack = [&](const uint8_t* v, int64_t& nulls) -> uint8_t* {
     nulls = 0;
@@ -197,7 +199,8 @@ void dnz_window::export_arrow(ArrowArray* out, ArrowSchema* schema, int32_t* has
   int64_t key_nulls = 0, agg_nulls = 0;
   uint8_t* kbm = pack(kvalid, key_nulls);
   uint8_t* abm = pack(avalid, agg_nulls);
-  b.add_child({kbm, koff, kbytes}, key_nulls);
+  if (key_width) b.add_child({kbm, kbytes}, key_nulls);
+  else b.add_child({kbm, koff, kbytes}, key_nulls);
   hand_out(b, ExportColumns{abm, agg_nulls, count, mn, mx, avg, sum, ws, we}, out, schema, has_output);
   for (auto& g : ranges) { g.r->exp_rows = g.r1; g.r->exp_bytes = g.b1; }
   if (blocking) {         // stream idle: drained sets can be recycled right away
@@ -209,18 +212,19 @@ void dnz_window::export_arrow(ArrowArray* out, ArrowSchema* schema, int32_t* has
 // again until n_rows == 0 when both sets may hold rows).  blocking: everything has been aggregated and the stream is idle, so
 // every emitted row is eligible.  Non-blocking: only rows whose emission is COMPLETE on the device; nothing queued is forced.
 // key_off entries are offsets into `key_bytes` (the set's byte buffer); key_bytes_len is the offset at which the last returned
-// key ends.
+// key ends.  Integer keys: key_off = NULL, key_bytes = the values of the returned rows (key_width bytes each, the NULL key's
+// zero-filled), key_bytes_len = n_rows * key_width.
 void dnz_window::export_device(dnz_device_result* out, bool blocking) {
   if (ungrouped) fail(DNZ_ERR_UNSUPPORTED, "ungrouped windows finish on the host (Final stage): use dnz_window_poll / dnz_window_poll_ready");
   memset(out, 0, sizeof *out);
-  ResultSet* r = nullptr; uint64_t r0 = 0, r1 = 0, b1 = 0;
+  ResultSet* r = nullptr; uint64_t r0 = 0, r1 = 0, b0 = 0, b1 = 0;
   if (blocking) fetch_ctl();
   else verify_completed();          // release the input of launches that have completed (never waits)
   for (int k = 0; k < 2 && !r; k++) {
     ResultSet& c = rs[k == 0 ? (wr ^ 1) : wr];
     uint64_t rows = c.rows, bytes = c.bytes;
     if (!blocking && !ready_rows(c, rows, bytes)) continue;
-    if (rows > c.exp_rows) { r = &c; r0 = c.exp_rows; r1 = rows; b1 = bytes; }
+    if (rows > c.exp_rows) { r = &c; r0 = c.exp_rows; r1 = rows; b0 = c.exp_bytes; b1 = bytes; }
   }
   if (!r) return;
   r->exp_rows = r1; r->exp_bytes = b1;
@@ -229,6 +233,7 @@ void dnz_window::export_device(dnz_device_result* out, bool blocking) {
   }
   out->n_rows = (int64_t)(r1 - r0); out->key_bytes_len = (int64_t)b1;
   out->key_off = r->key_off.as<int32_t>() + r0; out->key_bytes = r->key_bytes.as<uint8_t>(); out->key_valid = r->key_valid.as<uint8_t>() + r0;
+  if (key_width) { out->key_off = nullptr; out->key_bytes += b0; out->key_bytes_len = (int64_t)(b1 - b0); }
   out->count = r->count.as<int64_t>() + r0; out->min = r->mn.as<double>() + r0; out->max = r->mx.as<double>() + r0;
   out->avg = r->avg.as<double>() + r0; out->sum = r->sum.as<double>() + r0; out->agg_valid = r->agg_valid.as<uint8_t>() + r0;
   out->window_start_ms = r->wstart.as<int64_t>() + r0; out->window_end_ms = r->wend.as<int64_t>() + r0;

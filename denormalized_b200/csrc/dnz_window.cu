@@ -93,7 +93,14 @@ void dnz_window::init(const dnz_window_config* c, const ArrowSchema* schema) {
     if (c->key_column < 0 || c->key_column >= n_input_cols) fail(DNZ_ERR_INVALID, "key_column out of range");
     key_col = c->key_column;
     const ArrowSchema* ks = schema->children[key_col];
-    if (strcmp(ks->format, "u") != 0) fail(DNZ_ERR_UNSUPPORTED, "group key column '%s' has format '%s'; only Utf8 keys are implemented", ks->name, ks->format);
+    // DataFusion's GroupValuesPrimitive for the integer types: one group per distinct value, NULL is a group of its own
+    const char* kf = ks->format ? ks->format : "";
+    if (ks->dictionary) fail(DNZ_ERR_UNSUPPORTED, "group key column '%s' is dictionary-encoded; dictionary keys are not implemented", ks->name);
+    key_type = -1;
+    for (int t = 0; t < N_KEY_TYPES; t++) if (strcmp(kf, KEY_TYPES[t].format) == 0) key_type = t;
+    if (key_type < 0) fail(DNZ_ERR_UNSUPPORTED, "group key column '%s' has format '%s'; only Utf8, Int64, Int32, UInt64 and UInt32 keys are implemented", ks->name, kf);
+    key_width = KEY_TYPES[key_type].width;
+    key_nullable = (ks->flags & ARROW_FLAG_NULLABLE) != 0;
     key_name = ks->name ? ks->name : "key";
   }
   val_col = -1;
@@ -260,6 +267,7 @@ void dnz_window::arena_trim() {
 void dnz_window::parse_ctl(const CtlBlock& h) {
   if (h.ts_err) fail(DNZ_ERR_DATA, "a timestamp string does not match the format (the reference unwraps the parse error and panics)");
   if (const uint32_t xe = h.merge_err) {
+    if (xe & 8u) fail(DNZ_ERR_INVALID, "pane exchange: a rank sent keys of another type than this operator's group key (every rank must group by the same key type)");
     if (xe & 0x100u) fail(DNZ_ERR_NOMEM, "exchange ring overflow: an owner's ring is smaller than one step's packets (dnz_group_config.ring_entries / ring_key_bytes)");
     fail(DNZ_ERR_NOMEM, "pane merge failed (flags %u): the dictionary / key arena of this rank is too small for the keys it owns (in exchange mode expected_groups must cover the GLOBAL key set)", xe);
   }
@@ -291,7 +299,7 @@ uint32_t dnz_window::groups_bound() const {
 }
 uint64_t dnz_window::key_bytes_bound() const {
   const uint64_t fresh = groups_bound() - std::min<uint32_t>(groups_bound(), n_groups_host);
-  return key_bytes_total_host + fresh * INLINE_KEY + (arena_cap - std::min<uint64_t>(arena_used_host, arena_cap));
+  return key_bytes_total_host + fresh * INLINE_KEY + (arena_cap - std::min<uint64_t>(arena_used_host, arena_cap)) + key_width;   // + the NULL key's value (integer keys)
 }
 
 std::unique_ptr<Pane> dnz_window::new_pane(int64_t id) {
@@ -447,7 +455,12 @@ void dnz_window::push_host(ArrowArray* batch) {
     pb.d.val = (const double*)copy_in((const double*)buf_at(val, 1) + vo, (size_t)n * 8);
     copy_bitmap(val, vo, pb.d.val_valid, pb.d.val_vbit);
     // keys
-    if (!ungrouped) {
+    if (!ungrouped && key_width) {         // integer keys: the values (one per row, naturally aligned in the arena) and the bitmap
+      const int64_t ko = po + key->offset;
+      pb.d.bytes = (const uint8_t*)copy_in((const uint8_t*)buf_at(key, 1) + ko * key_width, (size_t)n * key_width);
+      pb.d.off = nullptr;
+      copy_bitmap(key, ko, pb.d.key_valid, pb.d.key_vbit);
+    } else if (!ungrouped) {
     int64_t ko = po + key->offset;
     const int32_t* hoff = (const int32_t*)buf_at(key, 1) + ko;
     pb.d.off = (const int32_t*)copy_in(hoff, (size_t)(n + 1) * 4);
@@ -474,7 +487,10 @@ void dnz_window::push_dev(const dnz_device_batch* b, int64_t nb) {
     const dnz_device_batch& s = b[i];
     if (s.n_rows < 0) fail(DNZ_ERR_INVALID, "device batch %lld: negative row count", (long long)i);
     if (s.n_rows >= (1ll << 31)) fail(DNZ_ERR_UNSUPPORTED, "batch with >= 2^31 rows");
-    if (s.n_rows > 0 && (!s.ts || !s.val || (!ungrouped && (!s.key_off || !s.key_bytes)))) fail(DNZ_ERR_INVALID, "device batch %lld: null column pointer", (long long)i);
+    if (s.n_rows > 0 && (!s.ts || !s.val || (!ungrouped && ((!key_width && !s.key_off) || !s.key_bytes)))) fail(DNZ_ERR_INVALID, "device batch %lld: null column pointer", (long long)i);
+    if (key_width && s.key_off) fail(DNZ_ERR_INVALID, "device batch %lld: key_off must be NULL for an integer key column (key_bytes holds the values)", (long long)i);
+    if (key_width && (reinterpret_cast<uintptr_t>(s.key_bytes) % (uintptr_t)key_width) != 0)
+      fail(DNZ_ERR_INVALID, "device batch %lld: integer key values must be aligned to their width (%d B)", (long long)i, key_width);
     if (cur().rows > 0 && cur().rows + s.n_rows > max_rows) seal_current();
     Slot& c = cur();
     PendingBatch pb;
@@ -641,7 +657,7 @@ dnz_window::RunGeom dnz_window::run_geometry(Slot& s, const std::vector<BatchMin
     const BatchMinMax& b = mm[i];
     const int64_t nr = s.bds[i].n_rows;
     if (nr == 0) continue;
-    g.rows += nr; g.alg_bytes += 20.0 * nr + (double)b.key_bytes;
+    g.rows += nr; g.alg_bytes += (key_width ? 16.0 + key_width : 20.0) * nr + (double)b.key_bytes;    // see dnz_stats
     fast += b.n_fast; generic += b.n_tiles - b.n_fast;
     if (s.bds[i].val_valid) g.val_nulls = true;
     if (b.n_valid == 0) continue;
@@ -737,8 +753,8 @@ void dnz_window::launch_aggregate_pass(Slot& s, const RunGeom& g, AggParams& P, 
   s.timed = (cfg.flags & DNZ_FLAG_KERNEL_TIMING) != 0; s.alg_bytes = g.alg_bytes;
   if (s.timed) CK(cudaEventRecord(s.ev0, stream));
   if (ungrouped) CK(launch_aggregate_ungrouped(P, sm_count, stream));
-  else if (cfg.flags & DNZ_FLAG_FORCE_GENERIC) CK(launch_aggregate_generic(P, sm_count, stream));
-  else CK(launch_aggregate(P, sm_count, stream));
+  else if (cfg.flags & DNZ_FLAG_FORCE_GENERIC) CK(launch_aggregate_generic(P, key_width, sm_count, stream));
+  else CK(launch_aggregate(P, key_width, sm_count, stream));
   if (use_priv) { CK(launch_merge_private(P, agg_grid, stream)); stats.total_launches++; }
   if (s.timed) CK(cudaEventRecord(s.ev1, stream));
   stats.agg_launches++; stats.total_launches++;
@@ -779,7 +795,7 @@ void dnz_window::resolve_deferred(Slot& s, const RunGeom& g, bool dirty, int64_t
     if (flags & (DEFER_NEED_FZ | DEFER_NEED_NULLROWS)) for_each_live_pane([&](Pane* p) { ensure_side_arrays(p); });
     const int out_list = in_list ^ 1;
     AggParams P = build_agg_params(s, g, dirty, horizon, out_list);
-    CK(launch_deferred(P, s.d_defer[in_list].as<DeferEntry>(), n_in, stream));   // replays the rows of the previous pass
+    CK(launch_deferred(P, key_width, s.d_defer[in_list].as<DeferEntry>(), n_in, stream));   // replays the rows of the previous pass
     stats.total_launches++;
     fetch_ctl();
     const SlotCtl& h = h_small.as<CtlBlock>()->slot[s.idx];
@@ -984,7 +1000,7 @@ void dnz_window::emit_windows(const std::vector<int64_t>& starts, const std::map
     if (k == 0) continue;
     E.n_panes = k; E.has_filter = cfg.has_filter;
     E.filter_col = cfg.has_filter ? aggs[cfg.filter_agg].kind : 0; E.filter_op = cfg.filter_op; E.filter_lit = cfg.filter_literal;
-    E.wstart = s; E.wend = s + L; E.n_groups = ng; E.rank = rank; E.world = world;
+    E.wstart = s; E.wend = s + L; E.n_groups = ng; E.key_width = key_width; E.rank = rank; E.world = world;
     E.dict = dict_view();
     E.gate = gate ? ctl()->slot : nullptr;
     E.blocked = gate ? &ctl()->slot[gate->idx].emit_blocked : nullptr;
@@ -1009,7 +1025,8 @@ void dnz_window::emit_windows(const std::vector<int64_t>& starts, const std::map
 namespace {
 struct CkptHeader {
   char magic[8];                 // "DNZCKPT1"
-  int64_t window_ms, slide_ms; int32_t n_aggs, flags;          // flags: 1 has_wm, 2 need_nullrows, 4 need_fz, 8 has_lwm
+  int64_t window_ms, slide_ms; int32_t n_aggs, flags;          // flags: 1 has_wm, 2 need_nullrows, 4 need_fz, 8 has_lwm,
+                                                               //   bits 4-7 the key type (KEY_TYPES: 0 = Utf8)
   int64_t wm, emitted_upto, next_seq, lwm, exported_pane_upto;
   uint32_t n_groups, null_gid_plus1; uint64_t arena_used, key_bytes_total;
   int64_t n_panes;
@@ -1026,7 +1043,7 @@ void dnz_window::checkpoint(std::vector<char>& blob) {
   CkptHeader H; memset(&H, 0, sizeof H);
   memcpy(H.magic, "DNZCKPT1", 8);
   H.window_ms = L; H.slide_ms = S; H.n_aggs = (int32_t)aggs.size();
-  H.flags = (has_wm ? 1 : 0) | (need_nullrows ? 2 : 0) | (need_fz ? 4 : 0) | (has_lwm ? 8 : 0);
+  H.flags = (has_wm ? 1 : 0) | (need_nullrows ? 2 : 0) | (need_fz ? 4 : 0) | (has_lwm ? 8 : 0) | (key_type << 4);      // Utf8 (0): the blob is what it was before integer keys
   H.wm = wm; H.emitted_upto = emitted_upto; H.next_seq = next_seq; H.lwm = lwm; H.exported_pane_upto = exported_pane_upto;
   H.n_groups = n_groups_host; H.null_gid_plus1 = h_small.as<CtlBlock>()->dict.null_gid;
   H.arena_used = std::min<uint64_t>(arena_used_host, arena_cap); H.key_bytes_total = key_bytes_total_host;
@@ -1055,6 +1072,7 @@ void dnz_window::restore(const char* blob, size_t bytes) {
   CkptHeader H; memcpy(&H, blob, sizeof H);
   if (memcmp(H.magic, "DNZCKPT1", 8) != 0) fail(DNZ_ERR_INVALID, "not a checkpoint blob");
   if (H.window_ms != L || H.slide_ms != S || H.n_aggs != (int32_t)aggs.size()) fail(DNZ_ERR_INVALID, "checkpoint was taken with another window / aggregate configuration");
+  if (((H.flags >> 4) & 0xF) != key_type) fail(DNZ_ERR_INVALID, "checkpoint was taken with another group key type");
   const size_t ng = H.n_groups, ab = round_up(H.arena_used, 8);
   const char* p = blob + sizeof H; const char* end = blob + bytes;
   auto need = [&](size_t n) { if ((size_t)(end - p) < n) fail(DNZ_ERR_INVALID, "checkpoint blob truncated"); };

@@ -258,6 +258,11 @@ struct dnz_window {
   dnz_window_config cfg{};
   std::vector<dnz_agg> aggs; std::vector<std::string> aliases;
   std::string key_name;
+  // group key type: an index into KEY_TYPES (0 Utf8; Int64 / Int32 / UInt64 / UInt32, whose values are key_width = 8 or 4 bytes
+  // each); key_width == 0 for Utf8 keys and for the ungrouped window.  key_nullable: the input field's nullability (integer keys
+  // echo it in the emitted schema; Utf8 keys are emitted nullable, as they always were)
+  int key_type = 0, key_width = 0; bool key_nullable = true;
+  uint32_t key_tag() const { return (uint32_t)key_type << KEY_TYPE_SHIFT; }
   int key_col = -1, val_col = -1, meta_col = -1, ts_child = -1, n_input_cols = 0;
   int ts_source = DNZ_TS_CANONICAL, ts_col = -1; TsFormat ts_fmt{};      // input-contract producer (SURVEY §8 f1)
   int dev = 0; int sm_count = 148;

@@ -59,8 +59,12 @@ typedef struct {
 typedef struct {
   uint32_t abi_version;      /* DNZ_ABI_VERSION                                                     */
   int32_t device;            /* CUDA device ordinal                                                 */
-  int32_t key_column;        /* top-level index of the Utf8 group-key column (one plain column,
-                                planner/streaming_window.rs:36-66), or DNZ_NO_KEY: the ungrouped window --
+  int32_t key_column;        /* top-level index of the group-key column (one plain column,
+                                planner/streaming_window.rs:36-66) of Arrow format "u" (Utf8), "l" (Int64),
+                                "i" (Int32), "L" (UInt64) or "I" (UInt32) -- integer keys group as DataFusion's
+                                GroupValuesPrimitive does: one group per distinct value, NULL a group of its own; the
+                                emitted key column has the input's type and nullability (a Utf8 key column
+                                is emitted nullable) -- or DNZ_NO_KEY: the ungrouped window --
                                 one partition of the Partial -> Final chain the planner builds for an empty
                                 group_by (planner/streaming_window.rs:133-153; WindowAggStream
                                 streaming_window.rs:640-828 on the device, FullWindowAggStream :882-1051 on
@@ -95,15 +99,18 @@ typedef struct dnz_window dnz_window;
 
 /* One RecordBatch whose needed column buffers are already resident in device memory (the
  * Arrow<->device buffer manager's output format; also what dnz_synth_generate produces).
- * Validity bitmaps: Arrow LSB-first, NULL = no nulls, bit 0 = row 0. */
+ * Validity bitmaps: Arrow LSB-first, NULL = no nulls, bit 0 = row 0.
+ * Utf8 keys: key_off holds n_rows+1 offsets into key_bytes.  Integer keys: key_off must be NULL and key_bytes points at the
+ * n_rows values (4 or 8 bytes each, aligned to their width); a non-NULL key_off is DNZ_ERR_INVALID. */
 typedef struct {
   int64_t n_rows;
   const int64_t* ts;        const uint8_t* ts_valid;    /* _streaming_internal_metadata.canonical_timestamp (ms) */
   const double* val;        const uint8_t* val_valid;   /* aggregate argument                                     */
-  const int32_t* key_off;   const uint8_t* key_bytes;   const uint8_t* key_valid;  /* Utf8 key: n_rows+1 offsets */
+  const int32_t* key_off;   const uint8_t* key_bytes;   const uint8_t* key_valid;  /* Utf8 key: n_rows+1 offsets; integer: NULL */
 } dnz_device_batch;
 
-/* Emitted rows, device resident (valid until the next call on the handle). */
+/* Emitted rows, device resident (valid until the next call on the handle).  Integer keys: key_off = NULL, key_bytes = the
+ * n_rows values (the input's width; a NULL key's value is zero), key_bytes_len = n_rows * width. */
 typedef struct {
   int64_t n_rows;
   int64_t key_bytes_len;
@@ -123,7 +130,8 @@ typedef struct {
   int64_t agg_launches;         /* aggregate-kernel launches                             */
   int64_t total_launches;       /* all kernel launches issued by the handle              */
   double agg_kernel_ms;         /* sum of aggregate-kernel durations (DNZ_FLAG_KERNEL_TIMING) */
-  double agg_algorithmic_bytes; /* 8 ts + 8 val + 4 offset + key bytes, summed over rows of timed launches */
+  double agg_algorithmic_bytes; /* 8 ts + 8 val + 4 offset + key bytes (integer keys: 8 ts + 8 val + key width), summed over
+                                   rows of timed launches */
   int64_t h2d_bytes; int64_t d2h_bytes;
   int64_t deferred_rows;        /* rows replayed after a table grew                      */
   int64_t generic_tiles; int64_t fast_tiles;
@@ -298,10 +306,11 @@ int32_t dnz_memcpy(void* dst, const void* src, int64_t bytes, int32_t kind);
  * buffers belong to the returned arena handle and are freed by dnz_synth_free. */
 typedef struct dnz_synth dnz_synth;
 int32_t dnz_synth_generate(int32_t device, int64_t row0, int64_t n_rows, int64_t batch_rows, uint64_t seed,
-                           int64_t groups, int64_t rows_per_ms, int64_t t0_ms, int32_t uuid_keys,
+                           int64_t groups, int64_t rows_per_ms, int64_t t0_ms,
+                           int32_t key_kind,  /* 0 "sensor_<id>" (Utf8), 1 a UUID string per id (Utf8), 2 Int64 keys = id */
                            int64_t key_mul, int64_t key_add, /* key id = id * key_mul + key_add (rank sharding) */
                            dnz_synth** arena, dnz_device_batch* out, int64_t n_batches);
-int64_t dnz_synth_bytes(const dnz_synth* arena);   /* algorithmic bytes held: 20*rows + key bytes */
+int64_t dnz_synth_bytes(const dnz_synth* arena);   /* algorithmic bytes held: 20*rows + key bytes (Int64 keys: 24*rows) */
 void dnz_synth_free(dnz_synth* arena);
 
 #ifdef __cplusplus

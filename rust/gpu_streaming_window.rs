@@ -7,7 +7,7 @@
 //!
 //! Plug-in point: `StreamingWindowPlanner::plan_extension` (`crates/core/src/planner/streaming_window.rs:154-165`)
 //! constructs `GpuStreamingWindowExec::try_new(..)` with exactly the arguments it passes to
-//! `StreamingWindowExec::try_new` today when the plan is GPU-eligible (one Utf8 group column; count/min/max/avg/sum over
+//! `StreamingWindowExec::try_new` today when the plan is GPU-eligible (one group column of type Utf8, Int64, Int32, UInt64 or UInt32; count/min/max/avg/sum over
 //! one Float64 column; window length in whole seconds, length % slide == 0) and returns an error otherwise --
 //! there is no CPU fallback inside the GPU operator.
 
@@ -211,6 +211,13 @@ impl ExecutionPlan for GpuStreamingWindowExec {
         let in_schema = self.input.schema();
         let ffi_schema = FFI_ArrowSchema::try_from(in_schema.as_ref())?;
         let key_column = in_schema.index_of(self.group_by.expr()[0].1.as_str())? as i32;
+        {   // the key types the library groups by (dnz_window_config.key_column); the integer types as GroupValuesPrimitive does
+            use arrow::datatypes::DataType;
+            let t = in_schema.field(key_column as usize).data_type();
+            if !matches!(t, DataType::Utf8 | DataType::Int64 | DataType::Int32 | DataType::UInt64 | DataType::UInt32) {
+                return Err(DataFusionError::NotImplemented(format!("GPU streaming window: group key of type {t}")));
+            }
+        }
         let aliases: Vec<std::ffi::CString> = self.aggr_expr.iter().map(|a| std::ffi::CString::new(a.name()).unwrap()).collect();
         let aggs: Vec<DnzAgg> = self.aggr_expr.iter().zip(&aliases).map(|(a, alias)| DnzAgg {
             kind: match a.fun().name() { "count" => 0, "min" => 1, "max" => 2, "avg" => 3, "sum" => 4, _ => -1 },
