@@ -42,8 +42,12 @@ void dnz_window::ungrouped_emit_run(Slot* sl, const std::vector<BatchMinMax>* mm
   }
   if (!wins.empty()) {
     const size_t n = wins.size();
-    if (n > u_ring) fail(DNZ_ERR_UNSUPPORTED, "%zu windows closed by one run (limit %zu)", n, u_ring);
     if (u_head + n > u_ring) { ungrouped_collect(true); u_head = 0; }              // staging full: take in what is on its way first
+    if (n > u_ring) {                                  // a run may close up to MAX_RUN_PANES windows: grow the staging, now idle
+      u_ring = std::max(n, 2 * u_ring);
+      d_uwins.alloc(u_ring * sizeof(UWindow)); d_ustates.alloc(u_ring * sizeof(UState));
+      h_uwins.reserve(u_ring * sizeof(UWindow)); h_ustates.reserve(u_ring * sizeof(UState));
+    }
     const size_t at = u_head;
     UWindow* hw = h_uwins.as<UWindow>() + at;
     for (size_t i = 0; i < n; i++) {

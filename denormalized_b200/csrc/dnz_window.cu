@@ -299,7 +299,10 @@ uint32_t dnz_window::groups_bound() const {
 }
 uint64_t dnz_window::key_bytes_bound() const {
   const uint64_t fresh = groups_bound() - std::min<uint32_t>(groups_bound(), n_groups_host);
-  return key_bytes_total_host + fresh * INLINE_KEY + (arena_cap - std::min<uint64_t>(arena_used_host, arena_cap)) + key_width;   // + the NULL key's value (integer keys)
+  // long keys can only be interned by launches the host has not seen complete (or by the owner's merge)
+  const bool interning = world > 1 || rows_since_known > 0;
+  const uint64_t arena_free = interning ? arena_cap - std::min<uint64_t>(arena_used_host, arena_cap) : 0;
+  return key_bytes_total_host + fresh * INLINE_KEY + arena_free + key_width;   // + the NULL key's value (integer keys)
 }
 
 std::unique_ptr<Pane> dnz_window::new_pane(int64_t id) {
@@ -982,9 +985,14 @@ void dnz_window::emit_normal(int64_t wm_new, Slot* gate) {
 // the launches do nothing (and raise that slot's emit-blocked flag) when any pipeline slot holds deferred rows at the time they run.
 void dnz_window::emit_windows(const std::vector<int64_t>& starts, const std::map<int64_t, Pane*>& src, Slot* gate) {
   if (starts.empty()) return;
-  const uint32_t ng = groups_bound();
+  uint32_t ng = groups_bound();
   if (ng == 0) return;
-  const uint64_t add_rows = (uint64_t)starts.size() * ng, add_bytes = (uint64_t)starts.size() * key_bytes_bound();
+  uint64_t add_rows = (uint64_t)starts.size() * ng, add_bytes = (uint64_t)starts.size() * key_bytes_bound();
+  if (R().bytes + add_bytes >= (1ull << 31)) {       // a bound per window adds up over thousands of windows: make it exact first
+    fetch_ctl();                                     // every enqueued launch done: no key can be interned before these emits
+    ng = groups_bound();
+    add_rows = (uint64_t)starts.size() * ng; add_bytes = (uint64_t)starts.size() * key_bytes_bound();
+  }
   ensure_result_capacity(add_rows, add_bytes);
   for (int64_t s : starts) {
     EmitParams E; memset(&E, 0, sizeof E);

@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _SO = os.path.join(_HERE, "_build", "libdnz_oracle.so")
 
 OPS = {">": 0, ">=": 1, "<": 2, "<=": 3, "==": 4, "!=": 5}
-COLS = {"count": 0, "min": 1, "max": 2, "average": 3, "avg": 3}
+COLS = {"count": 0, "min": 1, "max": 2, "average": 3, "avg": 3, "sum": 4}
 
 
 def build(force: bool = False) -> str:
@@ -46,7 +46,7 @@ class _Result(C.Structure):
     _fields_ = [("n", C.c_int64), ("key_off", C.c_void_p), ("key_bytes", C.c_void_p), ("key_isnull", C.c_void_p),
                 ("count", C.c_void_p), ("min", C.c_void_p), ("max", C.c_void_p), ("avg", C.c_void_p),
                 ("agg_isnull", C.c_void_p), ("window_start_ms", C.c_void_p), ("window_end_ms", C.c_void_p),
-                ("emit_seq", C.c_void_p)]
+                ("emit_seq", C.c_void_p), ("sum", C.c_void_p)]
 
 
 _lib = None
@@ -132,8 +132,9 @@ def _mkcfg(window_ms, slide_ms=0, filt=None) -> _Config:
     return c
 
 
-def _rows(res: _Result):
-    """-> list of tuples (window_start, window_end, key(bytes|None), count, min|None, max|None, avg|None, emit_seq)"""
+def _rows(res: _Result, with_sum=False):
+    """-> list of tuples (window_start, window_end, key(bytes|None), count, min|None, max|None, avg|None, emit_seq), with sum|None
+    appended at index 8 when `with_sum`"""
     n = res.n
     if n == 0:
         return []
@@ -147,18 +148,22 @@ def _rows(res: _Result):
     mn, mx, av = arr(res.min, np.float64, n), arr(res.max, np.float64, n), arr(res.avg, np.float64, n)
     anull = arr(res.agg_isnull, np.uint8, n)
     ws, we, seq = arr(res.window_start_ms, np.int64, n), arr(res.window_end_ms, np.int64, n), arr(res.emit_seq, np.int64, n)
+    sm = arr(res.sum, np.float64, n) if with_sum else None
     out = []
     for i in range(n):
         key = None if knull[i] else kb[off[i]:off[i + 1]]
         if anull[i]:
-            out.append((int(ws[i]), int(we[i]), key, int(cnt[i]), None, None, None, int(seq[i])))
+            r = (int(ws[i]), int(we[i]), key, int(cnt[i]), None, None, None, int(seq[i]))
         else:
-            out.append((int(ws[i]), int(we[i]), key, int(cnt[i]), float(mn[i]), float(mx[i]), float(av[i]), int(seq[i])))
+            r = (int(ws[i]), int(we[i]), key, int(cnt[i]), float(mn[i]), float(mx[i]), float(av[i]), int(seq[i]))
+        if with_sum:
+            r += (None if anull[i] else float(sm[i]),)
+        out.append(r)
     return out
 
 
 def _arrays(res: _Result) -> dict:
-    """Result set as numpy arrays (copies): key_off[n+1], key_bytes, key_isnull, count, min, max, avg, agg_isnull, window_start,
+    """Result set as numpy arrays (copies): key_off[n+1], key_bytes, key_isnull, count, min, max, avg, sum, agg_isnull, window_start,
     window_end.  For large outputs (millions of rows), where the tuple list of _rows() would take minutes."""
     n = int(res.n)
 
@@ -169,7 +174,7 @@ def _arrays(res: _Result) -> dict:
     off = arr(res.key_off, np.int32, n + 1) if n else np.zeros(1, np.int32)
     return {"n": n, "key_off": off, "key_bytes": arr(res.key_bytes, np.uint8, int(off[-1])), "key_isnull": arr(res.key_isnull, np.uint8, n),
             "count": arr(res.count, np.int64, n), "min": arr(res.min, np.float64, n), "max": arr(res.max, np.float64, n),
-            "avg": arr(res.avg, np.float64, n), "agg_isnull": arr(res.agg_isnull, np.uint8, n),
+            "avg": arr(res.avg, np.float64, n), "sum": arr(res.sum, np.float64, n), "agg_isnull": arr(res.agg_isnull, np.uint8, n),
             "window_start": arr(res.window_start_ms, np.int64, n), "window_end": arr(res.window_end_ms, np.int64, n)}
 
 
@@ -188,10 +193,11 @@ class OracleWindow:
             raise RuntimeError(self._L.orc_last_error(self._h).decode())
         return int(r)
 
-    def results(self, clear=True):
+    def results(self, clear=True, with_sum=False):
+        """Emitted rows (see _rows); `with_sum` appends sum at index 8."""
         res = _Result()
         self._L.orc_get_results(self._h, C.byref(res))
-        rows = _rows(res)
+        rows = _rows(res, with_sum)
         if clear:
             self._L.orc_clear_results(self._h)
         return rows
@@ -232,10 +238,10 @@ class OracleUngrouped:
             raise RuntimeError(self._L.orc_u_last_error(self._h).decode())
         return int(r)
 
-    def results(self, clear=True):
+    def results(self, clear=True, with_sum=False):
         res = _Result()
         self._L.orc_u_get_results(self._h, C.byref(res))
-        rows = _rows(res)
+        rows = _rows(res, with_sum)
         if clear:
             self._L.orc_u_clear_results(self._h)
         return rows
@@ -271,12 +277,12 @@ class OracleMT:
     def num_results(self) -> int:
         return int(self._L.orc_mt_num_results(self._h))
 
-    def results(self, clear=True):
+    def results(self, clear=True, with_sum=False):
         rows = []
         for p in range(self.partitions):
             res = _Result()
             self._L.orc_mt_get_results(self._h, p, C.byref(res))
-            rows += _rows(res)
+            rows += _rows(res, with_sum)
         if clear:
             self._L.orc_mt_clear_results(self._h)
         return rows

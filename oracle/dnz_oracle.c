@@ -252,21 +252,21 @@ static void frame_push(frame_t* f, const orc_batch* b) {
 typedef struct {
   int64_t n, cap, bytes, bytes_cap;
   int32_t* key_off; uint8_t* key_bytes; uint8_t* key_isnull;
-  int64_t* count; double* mn; double* mx; double* avg; uint8_t* agg_isnull;
+  int64_t* count; double* mn; double* mx; double* avg; double* sum; uint8_t* agg_isnull;
   int64_t* ws; int64_t* we; int64_t* seq;
 } results_t;
 
 static void results_free(results_t* r) {
-  free(r->key_off); free(r->key_bytes); free(r->key_isnull); free(r->count); free(r->mn); free(r->mx); free(r->avg);
+  free(r->key_off); free(r->key_bytes); free(r->key_isnull); free(r->count); free(r->mn); free(r->mx); free(r->avg); free(r->sum);
   free(r->agg_isnull); free(r->ws); free(r->we); free(r->seq); memset(r, 0, sizeof(*r));
 }
 static void results_push(results_t* r, const uint8_t* key, int32_t len, int key_isnull, int64_t count, double mn, double mx,
-                         double avg, int agg_isnull, int64_t ws, int64_t we, int64_t seq) {
+                         double avg, double sum, int agg_isnull, int64_t ws, int64_t we, int64_t seq) {
   if (r->n + 1 > r->cap) {
     int64_t c = r->cap ? r->cap * 2 : 1024;
     r->key_off = xrealloc(r->key_off, (c + 1) * 4); r->key_isnull = xrealloc(r->key_isnull, c);
     r->count = xrealloc(r->count, c * 8); r->mn = xrealloc(r->mn, c * 8); r->mx = xrealloc(r->mx, c * 8);
-    r->avg = xrealloc(r->avg, c * 8); r->agg_isnull = xrealloc(r->agg_isnull, c);
+    r->avg = xrealloc(r->avg, c * 8); r->sum = xrealloc(r->sum, c * 8); r->agg_isnull = xrealloc(r->agg_isnull, c);
     r->ws = xrealloc(r->ws, c * 8); r->we = xrealloc(r->we, c * 8); r->seq = xrealloc(r->seq, c * 8);
     if (r->cap == 0) r->key_off[0] = 0;
     r->cap = c;
@@ -276,7 +276,7 @@ static void results_push(results_t* r, const uint8_t* key, int32_t len, int key_
   r->bytes += len;
   int64_t i = r->n++;
   r->key_off[i + 1] = (int32_t)r->bytes; r->key_isnull[i] = (uint8_t)key_isnull;
-  r->count[i] = count; r->mn[i] = mn; r->mx[i] = mx; r->avg[i] = avg; r->agg_isnull[i] = (uint8_t)agg_isnull;
+  r->count[i] = count; r->mn[i] = mn; r->mx[i] = mx; r->avg[i] = avg; r->sum[i] = sum; r->agg_isnull[i] = (uint8_t)agg_isnull;
   r->ws[i] = ws; r->we[i] = we; r->seq[i] = seq;
 }
 
@@ -311,6 +311,7 @@ void orc_get_results(orc_window* w, orc_result* o) {
   o->n = w->res.n; o->key_off = w->res.key_off ? w->res.key_off : zero_off; o->key_bytes = w->res.key_bytes;
   o->key_isnull = w->res.key_isnull; o->count = w->res.count; o->min = w->res.mn; o->max = w->res.mx; o->avg = w->res.avg;
   o->agg_isnull = w->res.agg_isnull; o->window_start_ms = w->res.ws; o->window_end_ms = w->res.we; o->emit_seq = w->res.seq;
+  o->sum = w->res.sum;
 }
 
 /* snap_to_window_start (streaming_window.rs:1088-1094): whole-second arithmetic */
@@ -329,7 +330,7 @@ static frame_t* find_or_insert_frame(orc_window* w, int64_t start, int64_t end) 
   return w->frames[lo];
 }
 
-static int filter_pass(const orc_config* c, int64_t count, double mn, double mx, double avg, int agg_isnull) {
+static int filter_pass(const orc_config* c, int64_t count, double mn, double mx, double avg, double sum, int agg_isnull) {
   if (!c->has_filter) return 1;
   int cmp;
   if (c->filter_col == ORC_COL_COUNT) {
@@ -338,7 +339,7 @@ static int filter_pass(const orc_config* c, int64_t count, double mn, double mx,
     cmp = total_cmp((double)count, c->filter_lit);
   } else {
     if (agg_isnull) return 0;      /* null predicate -> row dropped */
-    double v = c->filter_col == ORC_COL_MIN ? mn : c->filter_col == ORC_COL_MAX ? mx : avg;
+    double v = c->filter_col == ORC_COL_MIN ? mn : c->filter_col == ORC_COL_MAX ? mx : c->filter_col == ORC_COL_SUM ? sum : avg;
     cmp = total_cmp(v, c->filter_lit);
   }
   switch (c->filter_op) {
@@ -354,9 +355,10 @@ static int64_t emit_frame(orc_window* w, frame_t* f) {
     int isnull = !f->mn_seen[g];                  /* NullState: null until first non-null value */
     double avg = isnull ? 0.0 : f->sum[g] / (double)f->avg_cnt[g];
     double mn = isnull ? 0.0 : f->mn[g], mx = isnull ? 0.0 : f->mx[g];
-    if (!filter_pass(&w->cfg, f->cnt[g], mn, mx, avg, isnull)) continue;
+    double sum = isnull ? 0.0 : f->sum[g];        /* sum(reading): PrimitiveGroupsAccumulator, +0.0 then += v in row order */
+    if (!filter_pass(&w->cfg, f->cnt[g], mn, mx, avg, sum, isnull)) continue;
     results_push(&w->res, f->g_bytes + f->g_off[g], f->g_off[g + 1] - f->g_off[g], (int32_t)g == f->null_gid,
-                 f->cnt[g], mn, mx, avg, isnull, f->start_ms, f->end_ms, w->seq);
+                 f->cnt[g], mn, mx, avg, sum, isnull, f->start_ms, f->end_ms, w->seq);
     emitted++;
   }
   return emitted;
@@ -709,6 +711,7 @@ void orc_u_get_results(orc_uwindow* w, orc_result* o) {
   o->n = w->res.n; o->key_off = w->res.key_off ? w->res.key_off : zero_off; o->key_bytes = w->res.key_bytes;
   o->key_isnull = w->res.key_isnull; o->count = w->res.count; o->min = w->res.mn; o->max = w->res.mx; o->avg = w->res.avg;
   o->agg_isnull = w->res.agg_isnull; o->window_start_ms = w->res.ws; o->window_end_ms = w->res.we; o->emit_seq = w->res.seq;
+  o->sum = w->res.sum;
 }
 /* PartialWindowAggFrame::push: rows with start <= ts < end; accumulators updated with the filtered batch */
 static void uframe_push(uframe_t* f, const orc_batch* b) {
@@ -775,7 +778,7 @@ int64_t orc_u_push(orc_uwindow* w, const orc_batch* b) {
           uframe_t* g = &w->ff[i];
           if (w->fwm > g->end) {
             int isnull = !g->has;
-            results_push(&w->res, NULL, 0, 1, (int64_t)g->cnt, isnull ? 0.0 : g->mn, isnull ? 0.0 : g->mx, isnull ? 0.0 : g->sum / (double)g->cnt, isnull, g->start, g->end, w->seq);
+            results_push(&w->res, NULL, 0, 1, (int64_t)g->cnt, isnull ? 0.0 : g->mn, isnull ? 0.0 : g->mx, isnull ? 0.0 : g->sum / (double)g->cnt, isnull ? 0.0 : g->sum, isnull, g->start, g->end, w->seq);
             emitted++;
           } else w->ff[k2++] = *g;
         }

@@ -27,7 +27,7 @@
  *   datafusion 42.0.0 (git probably-nothing-labs/arrow-datafusion @ d812edc, Cargo.toml:31):
  *     GroupValuesByes<i32>::intern (first-seen dense group ids, NULL key is its own group),
  *     CountGroupsAccumulator, PrimitiveGroupsAccumulator<Float64> min/max
- *     (start f64::MAX / f64::MIN, `if *cur > new` / `if *cur < new`), AvgGroupsAccumulator
+ *     (start f64::MAX / f64::MIN, `if *cur > new` / `if *cur < new`) and sum (start +0.0, += v in row order), AvgGroupsAccumulator
  *     (sum += v in row order; u64 count; sum / count), NullState, FilterExec.
  *   arrow-ord 53.3.0 cmp::{gt_eq,lt,gt,...}: floats compare with IEEE-754 totalOrder.
  */
@@ -40,7 +40,7 @@ extern "C" {
 #endif
 
 enum { ORC_OP_GT = 0, ORC_OP_GTE = 1, ORC_OP_LT = 2, ORC_OP_LTE = 3, ORC_OP_EQ = 4, ORC_OP_NEQ = 5 };
-enum { ORC_COL_COUNT = 0, ORC_COL_MIN = 1, ORC_COL_MAX = 2, ORC_COL_AVG = 3 };
+enum { ORC_COL_COUNT = 0, ORC_COL_MIN = 1, ORC_COL_MAX = 2, ORC_COL_AVG = 3, ORC_COL_SUM = 4 };
 
 typedef struct {
   int64_t window_ms;     /* window length (Duration, ms resolution)                       */
@@ -76,6 +76,7 @@ typedef struct {
   const uint8_t* agg_isnull;          /* byte per row: min/max/avg are null (group saw no non-null reading) */
   const int64_t* window_start_ms; const int64_t* window_end_ms;
   const int64_t* emit_seq;            /* index of the push() call that emitted the row */
+  const double* sum;                  /* sum(reading): +0.0 plus every non-null value in row order (null when agg_isnull) */
 } orc_result;
 
 orc_window* orc_create(const orc_config* cfg);

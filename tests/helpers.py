@@ -112,6 +112,44 @@ def to_record_batch(b: Batch):
     return make_record_batch(b.ts, b.val, b.key_off, b.key_bytes, b.ts_valid, b.val_valid, b.key_valid)
 
 
+SUM_AGGS = DEFAULT_AGGS + [("sum", "reading", "sum")]
+
+
+def same_f64(a, b):
+    """None == None, any NaN == any NaN, otherwise the same bits (+0.0 != -0.0)."""
+    if a is None or b is None:
+        return a is None and b is None
+    if math.isnan(a) or math.isnan(b):
+        return math.isnan(a) and math.isnan(b)
+    return bits(a) == bits(b)
+
+
+def assert_rows_exact(got, want, check_seq=False):
+    """Rows with sum at index 8 (OracleWindow.results(with_sum=True)): count / min / max / avg / sum all bit-exact, NaN as NaN."""
+    def key(r):
+        return (r[0], r[1], r[2] is None, r[2] or b"", (r[7] if check_seq else 0), r[3], bits(r[8]) or b"")
+    g, w = sorted(got, key=key), sorted(want, key=key)
+    assert len(g) == len(w), f"row count {len(g)} != {len(w)}"
+    for a, b in zip(g, w):
+        assert a[:4] == b[:4] and (not check_seq or a[7] == b[7]), f"{a} != {b}"
+        for i, name in ((4, "min"), (5, "max"), (6, "avg"), (8, "sum")):
+            assert same_f64(a[i], b[i]), f"{name} differs: {a} != {b}"
+
+
+def agg_rows(rb, aliases=("count", "min", "max", "average", "sum"), seq=0):
+    """Emitted RecordBatch -> rows (window_start, window_end, key, count, min, max, avg, seq, sum) read by the aliases of count, min,
+    max, avg and sum; the key is None when the batch has no key column (ungrouped), bytes otherwise (an integer v as str(v))."""
+    names = rb.schema.names
+    col = {name: rb.column(i) for i, name in enumerate(names)}
+    n = rb.num_rows
+    keyed = len(names) > len(aliases) + 2
+    keys = col[names[0]].cast("string").cast("binary").to_pylist() if keyed else [None] * n      # integer keys as str(v)
+    c, mn, mx, av, sm = (col[a].to_pylist() for a in aliases)
+    ws = col["window_start_time"].cast("int64").to_pylist()
+    we = col["window_end_time"].cast("int64").to_pylist()
+    return [(ws[i], we[i], keys[i], c[i], mn[i], mx[i], av[i], seq, sm[i]) for i in range(n)]
+
+
 def record_batch_rows(rb, seq=0):
     """Emitted RecordBatch (key|count|min|max|average|window_start_time|window_end_time) -> oracle-style row tuples."""
     cols = {name: rb.column(i) for i, name in enumerate(rb.schema.names)}
@@ -331,7 +369,7 @@ def concat_arrays(parts):
     out["key_bytes"] = np.concatenate([np.asarray(p["key_bytes"], np.uint8)[int(p["key_off"][0]): int(p["key_off"][len(p["count"])])] for p in parts])
     for k_out, k_a, k_b in [("key_isnull", "key_isnull", "key_valid"), ("agg_isnull", "agg_isnull", "agg_valid")]:
         out[k_out] = np.concatenate([np.asarray(p[k_a], np.uint8) if k_a in p else (np.asarray(p[k_b]) == 0).astype(np.uint8) for p in parts])
-    for k in ("count", "min", "max", "avg", "window_start"):
+    for k in ("count", "min", "max", "avg", "window_start") + (("sum",) if all("sum" in p for p in parts) else ()):
         out[k] = np.concatenate([np.asarray(p[k]) for p in parts])
     return out
 

@@ -71,10 +71,10 @@ class PyModel:
             fr = self.frames[s]
             if self.wm >= fr["end"]:
                 for key, st in fr["groups"].items():
-                    if st["seen"]:
-                        row = (s, fr["end"], key, st["cnt"], st["mn"], st["mx"], st["sum"] / st["cnt"], seq)
+                    if st["seen"]:     # sum(reading) is the avg state's sum: +0.0, then += v in row order
+                        row = (s, fr["end"], key, st["cnt"], st["mn"], st["mx"], st["sum"] / st["cnt"], seq, st["sum"])
                     else:
-                        row = (s, fr["end"], key, st["cnt"], None, None, None, seq)
+                        row = (s, fr["end"], key, st["cnt"], None, None, None, seq, None)
                     if self._pass(row):
                         self.out.append(row)
                 del self.frames[s]
@@ -83,7 +83,7 @@ class PyModel:
         if not self.filt:
             return True
         col, op, lit = self.filt
-        v = {"count": row[3], "min": row[4], "max": row[5], "average": row[6]}[col]
+        v = {"count": row[3], "min": row[4], "max": row[5], "average": row[6], "avg": row[6], "sum": row[8]}[col]
         if v is None:
             return False
         a, b = total_key(float(v)), total_key(float(lit))
@@ -102,7 +102,7 @@ class PyUngroupedModel:
                finalize_windows                       :926-951  frames with watermark > end, ascending start
     Row accumulators (DataFusion 42): count of non-null values; min / max of the non-null values under IEEE totalOrder, NULL when there
     are none; avg state (count, sum), merged by addition, evaluated as sum / count, NULL when no value was seen.
-    out rows: (window_start, window_end, None, count, min, max, avg, seq of the input batch that made the Final stage emit it)."""
+    out rows: (window_start, window_end, None, count, min, max, avg, seq of the input batch that made the Final stage emit it, sum)."""
 
     def __init__(self, L, S=0):
         self.L, self.S = L, S
@@ -163,5 +163,5 @@ class PyUngroupedModel:
             fr = self.final[s]
             if self.f_wm > fr["end"]:
                 avg = None if fr["sum"] is None else fr["sum"] / fr["cnt"]
-                self.out.append((fr["start"], fr["end"], None, fr["cnt"], fr["mn"], fr["mx"], avg, seq))
+                self.out.append((fr["start"], fr["end"], None, fr["cnt"], fr["mn"], fr["mx"], avg, seq, fr["sum"]))
                 del self.final[s]

@@ -247,3 +247,121 @@ def test_ungrouped_oracle_special_values_match_model():
     assert negz[3] == 20 and math.copysign(1.0, negz[4]) == -1.0 and math.copysign(1.0, negz[6]) == 1.0
     assert_rows_equal(got, m.out, check_seq=True)
     assert all(math.copysign(1.0, a[6]) == math.copysign(1.0, b[6]) for a, b in zip(got, m.out) if a[6] == 0.0)     # zero signs too
+
+
+# sum(reading): PrimitiveGroupsAccumulator (grouped) and SumAccumulator (ungrouped) -- +0.0, then += v; NULL when no value was seen
+def exact_rows(rng, n_batches, rows, n_keys, span_ms=300, null_frac=0.02):
+    """Rows whose values are k / 1024 with integer |k| <= 2^20: every partial sum is exact in f64, whatever the order."""
+    out, t = [], T0
+    for _ in range(n_batches):
+        b = []
+        for _ in range(rows):
+            k = int(rng.integers(-2 ** 20, 2 ** 20 + 1))
+            b.append((t + int(rng.integers(0, span_ms)), None if rng.random() < null_frac else k / 1024.0, b"k%d" % int(rng.integers(0, n_keys))))
+        out.append(b)
+        t += span_ms
+    return out
+
+
+def _window_sums(batches, L):
+    """{(window_start, key): exact integer sum of 1024 * v} of in-order tumbling windows, NULL values left out."""
+    acc = {}
+    for rows in batches:
+        for ts, v, k in rows:
+            if v is not None:
+                acc[(ts // L * L, k)] = acc.get((ts // L * L, k), 0) + int(v * 1024)
+    return acc
+
+
+@pytest.mark.parametrize("L,S", [(1000, 0), (4000, 1000)])
+def test_oracle_sum_matches_model_and_exact_integers(L, S):
+    from tests.helpers import assert_rows_exact
+    rng = np.random.default_rng(L + S)
+    batches = exact_rows(rng, 24, 60, 7)
+    batches.append([(T0 + 24 * 300 + 3 * L, 1.0, b"sentinel")])
+    o = OracleWindow(L, S)
+    for rows in batches:
+        o.push(rows_to_batch(rows))
+    got = o.results(with_sum=True)
+    assert len(got) > 20 and all(len(r) == 9 for r in got)
+    assert_rows_exact(got, run_model(batches, L, S), check_seq=True)      # avg too: sum and count are exact, so is the division
+    if S == 0:
+        exact = _window_sums(batches[:-1], L)
+        assert {(r[0], r[2]): r[8] for r in got} == {key: s / 1024.0 for key, s in exact.items()}
+
+
+def test_oracle_sum_against_pyarrow_group_by():
+    nb, n = 12, 4096
+    batches = [synth_batch(i * n, n, groups=50, rows_per_ms=8) for i in range(nb)]
+    for b in batches:                                   # exact values: k / 1024
+        b.val = np.round(b.val * 1024.0) / 1024.0 - 57.0
+    o = OracleWindow(1000)
+    for b in batches:
+        o.push(b)
+    o.push(rows_to_batch([(T0 + 60_000, 0.0, b"s")]))
+    got = {(r[0], r[2]): r[8] for r in o.results(with_sum=True)}
+    ts = np.concatenate([b.ts for b in batches])
+    keys = sum(([r[2] for r in batch_to_rows(b)] for b in batches), [])
+    tbl = pa.table({"w": (ts // 1000) * 1000, "k": pa.array(keys, pa.binary()), "v": np.concatenate([b.val for b in batches])})
+    agg = tbl.group_by(["w", "k"], use_threads=False).aggregate([("v", "sum")])
+    want = dict(zip(zip(agg["w"].to_pylist(), agg["k"].to_pylist()), agg["v_sum"].to_pylist()))
+    assert len(want) > 100 and got == want
+
+
+def test_oracle_sum_edges():
+    """NULL-only -> NULL; -0.0 only -> +0.0 (the state starts at +0.0); NaN; +inf with -inf -> NaN; +inf alone."""
+    import struct
+    nan, inf = float("nan"), float("inf")
+    per_key = {b"null": [None, None], b"negz": [-0.0, -0.0], b"z": [0.0, -0.0], b"nan": [1.5, nan], b"infs": [inf, -inf],
+               b"pinf": [inf, 2.0], b"ex": [0.5, 0.25, -0.125]}
+    rows = [(T0 + i, v, k) for k, vals in per_key.items() for i, v in enumerate(vals)]
+    close = [(T0 + 5000, 1.0, b"s")]
+    for run in (run_model, None):
+        if run is None:
+            o = OracleWindow(1000)
+            o.push(rows_to_batch(rows)); o.push(rows_to_batch(close))
+            out = {r[2]: r[8] for r in o.results(with_sum=True)}
+        else:
+            out = {r[2]: r[8] for r in run([rows, close], 1000)}
+        assert out[b"null"] is None
+        assert struct.pack("<d", out[b"negz"]) == struct.pack("<d", 0.0) and struct.pack("<d", out[b"z"]) == struct.pack("<d", 0.0)
+        assert math.isnan(out[b"nan"]) and math.isnan(out[b"infs"]) and out[b"pinf"] == inf and out[b"ex"] == 0.625
+    tbl = pa.table({"k": [k for k, vals in per_key.items() for _ in vals], "v": pa.array([v for vals in per_key.values() for v in vals], pa.float64())})
+    pa_sum = dict(zip(*[tbl.group_by("k", use_threads=False).aggregate([("v", "sum")])[c].to_pylist() for c in ("k", "v_sum")]))
+    assert pa_sum[b"null"] is None and pa_sum[b"ex"] == 0.625 and math.isnan(pa_sum[b"infs"]) and pa_sum[b"pinf"] == inf
+
+
+@pytest.mark.parametrize("op", [">", ">=", "<", "<=", "==", "!="])
+def test_oracle_sum_filter_matches_model(op):
+    rng = np.random.default_rng(11)
+    batches = exact_rows(rng, 12, 40, 5)
+    special = [(T0 + 1, 2.5, b"a"), (T0 + 2, -2.5, b"a"), (T0 + 3, -0.0, b"nz"), (T0 + 4, float("nan"), b"nan"),
+               (T0 + 5, float("inf"), b"inf"), (T0 + 6, None, b"null")]
+    batches[0] = batches[0] + special
+    batches.append([(T0 + 12 * 300 + 3000, 1.0, b"sentinel")])
+    o = OracleWindow(1000)
+    for rows in batches:
+        o.push(rows_to_batch(rows))
+    exact = next(r[8] for r in o.results(with_sum=True) if r[2] != b"a")
+    for lit in (exact, 0.0, -0.0, float("nan"), float("inf"), float("-inf")):
+        got, want = run_oracle(batches, 1000, filt=("sum", op, lit)), run_model(batches, 1000, filt=("sum", op, lit))
+        assert_rows_equal(got, want, rel=0.0, check_seq=True)
+        if lit == exact and op == "==":
+            assert got
+
+
+@pytest.mark.parametrize("L,S", [(1000, 0), (4000, 1000)])
+def test_ungrouped_oracle_sum_matches_model(L, S):
+    from oracle import OracleUngrouped
+    from tests.helpers import assert_rows_exact
+    from tests.pymodel import PyUngroupedModel
+    rng = np.random.default_rng(3 * L + S)
+    raw = exact_rows(rng, 40, 50, 1)
+    raw[5] = [(ts, None, k) for ts, _, k in raw[5]]
+    raw[9] = [(ts, -0.0, k) for ts, _, k in raw[9]]
+    o, m, got = OracleUngrouped(L, S), PyUngroupedModel(L, S), []
+    for rows in raw:
+        o.push(rows_to_batch(rows)); got += o.results(with_sum=True)
+        m.push(rows)
+    assert len(m.out) > 3
+    assert_rows_exact(got, m.out, check_seq=True)
